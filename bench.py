@@ -42,7 +42,7 @@ warnings.filterwarnings("ignore")
 METRIC = "variants/sec filtered+scored on 50M-record synthetic VCF"
 SEED = 20260922
 N_CUSTOM = 40
-FALLBACK_HBM_GBS = 6650.0
+FALLBACK_HBM_GBS = 3350.0  # H100 SXM data sheet (HBM3, 3.35 TB/s): used only where no measured peak is present
 
 
 def log(*a):
@@ -289,6 +289,35 @@ def cpu_baseline_sample(text: bytes, header_text: str, model, tr, customs) -> di
                     "reference spends less time in those stages", "_res": res}
 
 
+DUMP_SEED = 7
+DUMP_MAX_RECORDS = 1 << 20
+DUMP_MAX_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir: str, d_low, d_probs, d_qual, counts):
+    """What the caller of the device-resident path receives (FILTER flag, class probabilities, TREE_SCORE and the
+    pass/fail counters), for the same seeded sample of records in every run.  float32 / float64 only."""
+    import torch
+
+    n, k = d_probs.shape
+    per_record = 8 + 4 + 4 * k + 8  # index, low_score, probs, qual
+    m = min(n, DUMP_MAX_RECORDS, (DUMP_MAX_BYTES - 4096) // per_record)
+    idx = np.sort(np.random.default_rng(DUMP_SEED).choice(n, size=m, replace=False))
+    idx_t = torch.from_numpy(idx).to(d_low.device)
+    arrays = {
+        "record_index": idx.astype(np.float64),
+        "low_score": d_low.index_select(0, idx_t).cpu().numpy().astype(np.float32),
+        "probs": d_probs.index_select(0, idx_t).cpu().numpy().astype(np.float32),
+        "qual": d_qual.index_select(0, idx_t).cpu().numpy().astype(np.float64),
+        "counts": np.asarray(counts, dtype=np.float64),
+    }
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
+    log(f"[bench] outputs of the last step: {m} of {n} records -> {out_dir} "
+        f"({sum(a.nbytes for a in arrays.values()) / 2**20:.1f} MiB)")
+
+
 # ------------------------------------------------------------------------------------------
 def main():  # noqa: C901, PLR0912, PLR0915
     ap = argparse.ArgumentParser()
@@ -314,7 +343,12 @@ def main():  # noqa: C901, PLR0912, PLR0915
                     help="skip the file-to-file leg (BASELINE configs[1] through `ugvc filter_variants_pipeline`, N=1 only)")
     ap.add_argument("--e2e-file-records", type=int, default=5_000_000)
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last device-resident step returned (rank 0's records) "
+                         "as DIR/<name>.npy: a fixed, seeded sample of at most 1 Mi records")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     if int(os.environ.get("WORLD_SIZE", "1")) == 1 and not args.no_e2e and not args.no_e2e_bgzf:
         args.e2e_bgzf = True
     claim_stdout()
@@ -447,13 +481,15 @@ def main():  # noqa: C901, PLR0912, PLR0915
         dist.all_reduce(t_el, op=dist.ReduceOp.MAX)
     elapsed_ms = float(t_el.item())
     value = args.records * args.steps / (elapsed_ms / 1e3)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, d_low, d_probs, d_qual, counts_total)
 
     # ---- roofline of the dominant kernel (this rank's launches)
     peaks_path = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(peaks_path):
         peak, peak_src = float(json.load(open(peaks_path))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     else:
-        peak, peak_src = FALLBACK_HBM_GBS, "fallback"
+        peak, peak_src = FALLBACK_HBM_GBS, "fallback: H100 SXM data-sheet HBM3 bandwidth, not a measured peak"
     names = ["k0_line_index", "k1_field_parse", "k2_feature_assembly", "k3_inference"]
     S, F = ctx.n_slots, ctx.n_features
     rec_per_launch = n_mine / len(batches)
@@ -469,9 +505,9 @@ def main():  # noqa: C901, PLR0912, PLR0915
     achieved = alg_bytes[dom] / (stage_ms[dom] / 1e3) / 1e9
     path_bytes = total_bytes / max(1, n_mine) + 4 * K + 9  # B_alg per record, SURVEY.md 8d
     kernels_ms_per_step = sum(stage_sum) / args.steps
-    # DRAM bytes per record of each kernel: read from the committed summary of the `ncu --set full` captures
-    # (profiles/ncu_traffic.json, written by scripts/save_profiles_r2.py from the .ncu-rep files: dram__bytes_read.sum +
-    # dram__bytes_write.sum of one launch and the records that launch parsed)
+    # DRAM bytes per record of each kernel, where a summary of `ncu --set full` captures taken on this GPU model is
+    # present (profiles/ncu_traffic.json: {kernel: {"dram_bytes": dram__bytes_read.sum + dram__bytes_write.sum of one
+    # launch, "records": the records that launch parsed}}); None otherwise
     traffic_path = os.path.join(ROOT, "profiles", "ncu_traffic.json")
     ncu_traffic = json.load(open(traffic_path)) if os.path.exists(traffic_path) else {}
     stage_kernel = {"k1_field_parse": "k1_tok", "k3_inference": "k3_heap", "k2_feature_assembly": "k2_features",

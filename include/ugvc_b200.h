@@ -1,5 +1,5 @@
 /*
- * ugvc_b200.h -- C ABI of the B200-native filter_variants_pipeline hot path.
+ * ugvc_b200.h -- C ABI of the H100-native (sm_90a) filter_variants_pipeline hot path.
  *
  * The reference (Ultimagen/VariantCalling, 100 % Python) has no FFI for this
  * path; its boundary is the CLI, the model pickle and the Python functions

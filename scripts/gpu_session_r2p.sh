@@ -1,5 +1,5 @@
 #!/bin/bash
-# Round-2 closing GPU session (about 4 minutes): the --treat_multiallelics kernels on a real B200.
+# Round-2 closing GPU session (about 4 minutes): the --treat_multiallelics kernels on a real GPU.
 #   gpurun --timeout 330 -- 'bash scripts/gpu_session_r2p.sh'
 # 1. their parity tests + the CLI tests of the branch (stops here when they fail: the remaining budget is for a re-test)
 # 2. memcheck of one small contig through the index pass, build and merge

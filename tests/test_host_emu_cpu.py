@@ -66,7 +66,7 @@ def test_two_rank_cli_run_equals_the_single_process_output(tmp_path):
             "--device", "0"]  # the emulation exposes one device (on a GPU box every rank takes LOCAL_RANK)
     for c in ds["customs"]:
         tool += ["--custom_annotations", c]
-    env = dict(os.environ, UGVC_LIB_PATH=EMU_LIB)
+    env = dict(os.environ, UGVC_LIB_PATH=EMU_LIB, CUDA_VISIBLE_DEVICES="")  # gloo: both ranks share emulated device 0
     env.pop("RANK", None), env.pop("WORLD_SIZE", None)
     one, two = str(tmp_path / "one.vcf.gz"), str(tmp_path / "two.vcf.gz")
     r1 = subprocess.run([sys.executable, "ugvc", *tool, "--output_file", one], cwd=ROOT, env=env, capture_output=True,
@@ -110,7 +110,7 @@ def test_two_rank_run_of_the_multiallelic_branch(tmp_path):
             "--recalibrate_genotype", "--device", "0"]
     for c in ds["customs"]:
         tool += ["--custom_annotations", c]
-    env = dict(os.environ, UGVC_LIB_PATH=EMU_LIB)
+    env = dict(os.environ, UGVC_LIB_PATH=EMU_LIB, CUDA_VISIBLE_DEVICES="")  # gloo: both ranks share emulated device 0
     env.pop("RANK", None), env.pop("WORLD_SIZE", None)
     one, two = str(tmp_path / "one.vcf.gz"), str(tmp_path / "two.vcf.gz")
     r1 = subprocess.run([sys.executable, "ugvc", *tool, "--output_file", one], cwd=ROOT, env=env, capture_output=True,

@@ -24,7 +24,7 @@ def main(argv=None):
         return 0 if len(argv) >= 2 else 1  # noqa: PLR2004
     tool = argv[1]
     if tool not in TOOLS:
-        print(f"ugvc: unknown tool {tool!r}; this B200 build provides: {', '.join(sorted(TOOLS))}", file=sys.stderr)
+        print(f"ugvc: unknown tool {tool!r}; this build provides: {', '.join(sorted(TOOLS))}", file=sys.stderr)
         return 2
     import importlib
 

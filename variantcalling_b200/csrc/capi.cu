@@ -63,7 +63,7 @@ struct Lane {
 
 struct ugvc_ctx {
     int device = 0;
-    int sm_count = 148;
+    int sm_count = 132;  // replaced by the device's count when the context opens
     std::string err;
     bool has_plan = false;
     DevPlan plan{};
@@ -622,7 +622,7 @@ extern "C" int ugvc_load_plan(ugvc_ctx* ctx, const void* blob, size_t n_bytes) {
     p.htab = ctx->d_htab;
     p.first_fixed_slot = first_fixed;
     if (k1_smem_bytes(p) > 227 * 1024 || k3_smem_bytes(p) > 227 * 1024 || !k3_plan_fits(p))
-        return fail(ctx, UGVC_E_PLAN, "plan needs more shared memory than one sm_100 CTA has");
+        return fail(ctx, UGVC_E_PLAN, "plan needs more shared memory than one sm_90 CTA has");
     if (h.model_kind != MODEL_LOGISTIC && h.model_kind != MODEL_NONE) {
         const uint32_t* root = reinterpret_cast<const uint32_t*>(hb + o_root);
         const unsigned cap = k3_chunk_nodes_cap(p);

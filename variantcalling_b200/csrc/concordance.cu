@@ -35,7 +35,7 @@
 
 struct ugvc_conc {
     int device = 0;
-    int sm_count = 148;
+    int sm_count = 132;  // replaced by the device's count when the handle opens
     cudaStream_t st = nullptr;
     std::string err;
     long long launches = 0;
@@ -421,7 +421,7 @@ extern "C" int ugvc_conc_classify(ugvc_conc* h, int64_t n, const int8_t* gt_ulti
     if (e == cudaSuccess && base_fn) e = cudaMemcpy(d_b, base_fn, n, cudaMemcpyHostToDevice);
     if (e == cudaSuccess) {
         int64_t blocks = (n + CONC_TPB - 1) / CONC_TPB;
-        if (blocks > 148 * 16) blocks = 148 * 16;
+        if (blocks > h->sm_count * 16) blocks = h->sm_count * 16;
         conc_classify_gt<<<(unsigned)blocks, CONC_TPB>>>(n, d_u, d_t, d_b, d_c, d_g);
         h->launches += 1;
         e = cudaGetLastError();

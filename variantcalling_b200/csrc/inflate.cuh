@@ -296,7 +296,7 @@ __host__ __device__ inline int inf_block(const uint8_t* in, uint32_t n_in, uint8
 #if defined(__CUDACC__) && !defined(UGVC_HOST_EMU)
 // ---------------------------------------------------------------------------------------------------
 // One WARP per BGZF block.  The thread-per-block decoder above diverges 32 ways inside a warp and keeps its
-// tables in local memory (measured: 7 GB/s of output on a B200).  Here the serial part -- bit buffer, table
+// tables in local memory.  Here the serial part -- bit buffer, table
 // look-up, symbol decode -- runs warp-uniformly (every lane holds the same state, the tables are in shared
 // memory, the input word is a broadcast load), so nothing diverges, and the byte moves of the matches are spread
 // over the lanes (lane k copies byte k; an overlapping match repeats with period d).  Literals are stored by

@@ -1,4 +1,4 @@
-// kernels.cu -- the hot path of filter_variants_pipeline as sm_100a CUDA kernels.
+// kernels.cu -- the hot path of filter_variants_pipeline as sm_90a (H100) CUDA kernels.
 //
 //   K0  line index      : one pass over the VCF text (decoupled look-back) -> line_start[], n_records
 //   K1  field parse     : one thread per record walks the 8 fixed columns, the INFO key=value
@@ -277,7 +277,7 @@ struct NumCur {
 
 // Bit 7 set in the FIRST byte of w that equals tab, newline or one of the two pattern bytes
 // (bytes above the first match may carry false positives -- only the lowest set bit is used).
-// Classic has-zero-byte SWAR on 64-bit words: sm_100 has no byte-compare instruction
+// Classic has-zero-byte SWAR on 64-bit words: sm_90 has no byte-compare instruction
 // (__vcmpeq4 is emulated with five instructions).
 __device__ __forceinline__ unsigned long long has_zero(unsigned long long x) {
     return (x - 0x0101010101010101ull) & ~x & 0x8080808080808080ull;
@@ -1542,7 +1542,6 @@ static K3hShape k3h_shape(const DevPlan& plan) {
     const bool forest = plan.h.model_kind != MODEL_LOGISTIC;
     const size_t all = forest ? (size_t)plan.h.n_trees * k3h_tree_bytes(plan) : 0;
     // two half-CTAs with one tile each first (most warps for the shared memory), then double-buffered single groups
-    // (measured on cfg 3: 448 threads x 8 trees in flight 0.372 ms per launch, 384 x 16 0.406 ms, 448 x 12 0.381 ms)
     const K3hShape cand[8] = {{512, 1, 2}, {448, 1, 2}, {384, 1, 2}, {256, 2, 1}, {192, 2, 1}, {128, 2, 1}, {256, 1, 1}, {128, 1, 1}};
     for (int i = 0; i < 8; ++i) {
         if (force >= 0 && i != force) continue;

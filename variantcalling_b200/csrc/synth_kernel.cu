@@ -16,6 +16,7 @@
 #include "../../include/ugvc_b200.h"
 
 int ugvc_ctx_device(const ugvc_ctx* ctx);
+int ugvc_ctx_sm_count(const ugvc_ctx* ctx);
 void ugvc_ctx_count_launches(ugvc_ctx* ctx, int n);
 cudaStream_t ugvc_ctx_default_stream(ugvc_ctx* ctx);
 int ugvc_ctx_fail(ugvc_ctx* ctx, int code, const char* msg);
@@ -347,7 +348,7 @@ extern "C" int ugvc_synth_device(ugvc_ctx* ctx, uint64_t seed, int64_t first_rec
     if (e != cudaSuccess) return ugvc_ctx_fail(ctx, UGVC_E_CUDA, cudaGetErrorString(e));
     unsigned long long* offs = lens + (n_records + 1);
     cudaMemsetAsync(lens + n_records, 0, sizeof(unsigned long long), st);
-    const int blocks = 148 * 8;
+    const int blocks = ugvc_ctx_sm_count(ctx) * 8;
     synth_lengths<<<blocks, 128, 0, st>>>(seed, first_record, n_records, total_records, n_custom, lens);
     cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, lens, offs, (int)(n_records + 1), st);
     e = cudaMalloc(&tmp, tmp_bytes ? tmp_bytes : 8);

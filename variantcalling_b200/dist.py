@@ -49,8 +49,7 @@ def allreduce_counts(counts_tensor, group=None):
 def bind_to_gpu_numa_node(gpu_index: int) -> dict:
     """Pin this process (and the threads it starts later) to the CPUs of the NUMA node the GPU hangs off, BEFORE any
     pinned host buffer is allocated: first-touch then places those buffers on that node, so the H2D / D2H copies of
-    several ranks do not all cross the same memory controller / PCIe root (round 1 measured 54 -> 36 GB/s per GPU at
-    four and eight ranks without it).  Best effort: returns what was done, never raises."""
+    several ranks do not all cross the same memory controller / PCIe root.  Best effort: returns what was done, never raises."""
     import os
     import subprocess
 

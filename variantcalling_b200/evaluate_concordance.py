@@ -63,7 +63,7 @@ def run(argv: list[str]):
     args = parse_args(argv)
     logging.basicConfig(format="%(asctime)s %(message)s", level=getattr(logging, args.verbosity))
     if args.output_bed:
-        raise NotImplementedError("--output_bed (BED files per classification) is not part of the B200 path")
+        raise NotImplementedError("--output_bed (BED files per classification) is not part of the device path")
     df = read_frame(args.input_file, args.dataset_key)
     score_column = args.score_key.lower()
     if score_column not in df.columns or all(df[score_column].isna()):

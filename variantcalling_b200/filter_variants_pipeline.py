@@ -1,5 +1,5 @@
 #!/env/python
-"""POST-GATK variant filtering -- B200-native drop-in for the reference tool.
+"""POST-GATK variant filtering -- H100-native drop-in for the reference tool.
 
 Mirrors ``ugbio_utils/src/filtering/ugbio_filtering/filter_variants_pipeline.py``:
 same flags (``parse_args``, :20-70), same ``run(argv)`` entry (argv without the
@@ -67,7 +67,7 @@ def parse_args(argv: list[str]) -> argparse.Namespace:
     ap_var.add_argument("--output_file", help="Output VCF file", type=str, required=True)
     ap_var.add_argument("--limit_to_contigs", help="Limit filtering to these contigs", nargs="+", type=str,
                         default=None)
-    # B200 host knobs (not in the reference; defaults need no tuning)
+    # host knobs (not in the reference; defaults need no tuning)
     ap_var.add_argument("--device", help="CUDA device index (default: LOCAL_RANK or 0)", type=int, default=None)
     ap_var.add_argument("--host_io", help="Inflate, edit and deflate the records on host threads even when the device-side "
                         "file path applies", action="store_true")

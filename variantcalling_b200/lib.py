@@ -447,8 +447,8 @@ def learn_key_order(sample: bytes, max_records: int = 2000, min_presence: float 
     graph is a common supersequence of all the records' key sequences (records written by
     GATK/htsjdk carry their keys sorted, optional keys simply missing).  Keys caught in a cycle
     (files mixing orders) are left out and take K1's generic lookup path, and so can keys present
-    in fewer than ``min_presence`` of the records (measured on B200: scheduling even the 15 %-present
-    annotations of the cfg-3 input is 10 % faster than leaving them to the generic path, hence 0)."""
+    in fewer than ``min_presence`` of the records (default 0: even the 15 %-present annotations of the cfg-3
+    input are scheduled rather than left to the generic path)."""
     import heapq
 
     first_seen: dict[str, int] = {}
