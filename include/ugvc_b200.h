@@ -380,6 +380,11 @@ int ugvc_ma_merge(ugvc_ma* h, const double* lik, int64_t n_rows, int n_classes, 
 /* Test hook: K3's xgboost-flavoured fp32 sigmoid evaluated on the device for an array of margins (p1 and the
  * exponential it used). */
 int ugvc_test_device_sigmoid(ugvc_ctx* ctx, const float* margins, int n, float* out_p1, float* out_e);
+/* Test hook: the K3 launch the loaded plan gets (also in the host emulation, which runs the same chunking).
+ * out = {kernel (0 k3_heap, 1 k3_infer), threads per CTA, tile buffers per group, groups per CTA (records per tile:
+ * threads / groups), trees one thread walks at once, forest chunk (k3_heap: trees, k3_infer: nodes; 0 for a linear
+ * model), 1 when the whole model is staged once, CTAs of the persistent grid}.  UGVC_E_STATE without a model. */
+int ugvc_test_k3_config(ugvc_ctx* ctx, int32_t out[8]);
 int ugvc_test_parse_float(const char* text, float* out_f32, double* out_f64, int* out_consumed);
 /* Test hook: the device BGZF encoder (csrc/deflate.cuh) run on the host on one block of at most 57344 bytes (4 readable
  * bytes after n); out receives a complete BGZF block (<= 65536 bytes), the size is returned. */

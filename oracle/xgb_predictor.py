@@ -51,6 +51,67 @@ def sklearn_gb_to_xgb_json(model) -> dict:
                         "gradient_booster": {"name": "gbtree", "model": {"trees": trees, "tree_info": info}}}}
 
 
+def random_gbtree_document(seed: int, x: np.ndarray, n_trees: int, *, num_class: int = 0, max_depth: int = 12,
+                           full_depth: bool = False, leaf_p: float = 0.3, tree_info="rounds",
+                           base_score: float = 0.5) -> dict:
+    """A random xgboost gbtree JSON document over the columns of ``x`` -- deep / large models without xgboost.
+
+    ``num_class`` 0 gives ``binary:logistic``, otherwise ``multi:softprob`` with that many classes (2 included).
+    Every tree has its own depth in [1, max_depth] (exactly ``max_depth`` with ``full_depth``), reached by one
+    random root-to-leaf path; off that path a node becomes a leaf with probability ``leaf_p``, so the trees are
+    unbalanced.  Nodes are numbered breadth first like xgboost's.  A split condition is a float32 value of its
+    column in ``x`` (rows then sit exactly on it); leaf values are float32.  ``tree_info``: "rounds" (class of
+    tree t = t % num_class, xgboost's layout), "blocks" (all trees of class 0, then class 1, ...), "shuffled" (a
+    seeded permutation of the rounds layout) or an explicit list."""
+    rng = np.random.default_rng(seed)
+    x = np.asarray(x, dtype=np.float32)
+    n_out = max(1, num_class)
+    trees = []
+    for _ in range(n_trees):
+        depth = max_depth if full_depth else int(rng.integers(1, max_depth + 1))
+        path = rng.integers(0, 2, size=depth)  # the branch taken at each level by the path that reaches `depth`
+        left, right, feat, cond = [], [], [], []
+        queue = [(0, True)]  # (level, on the deep path); index in the lists == breadth-first node id
+        left.append(-1), right.append(-1), feat.append(0), cond.append(0.0)
+        head = 0
+        while head < len(queue):
+            level, on_path = queue[head]
+            nid = head
+            head += 1
+            is_leaf = level == depth or (not on_path and rng.random() < leaf_p)
+            if is_leaf:
+                cond[nid] = float(np.float32(rng.normal(0.0, 0.4)))
+                continue
+            f = int(rng.integers(0, x.shape[1]))
+            feat[nid] = f
+            cond[nid] = float(x[int(rng.integers(0, x.shape[0])), f])
+            for side in (0, 1):
+                child = len(left)
+                left.append(-1), right.append(-1), feat.append(0), cond.append(0.0)
+                queue.append((level + 1, on_path and int(path[level]) == side))
+                if side == 0:
+                    left[nid] = child
+                else:
+                    right[nid] = child
+        trees.append({"left_children": left, "right_children": right, "split_indices": feat,
+                      "split_conditions": cond, "default_left": [0] * len(left), "base_weights": list(cond)})
+    if isinstance(tree_info, str):
+        rounds = [t % n_out for t in range(n_trees)] if num_class else [0] * n_trees
+        if tree_info == "rounds":
+            tree_info = rounds
+        elif tree_info == "blocks":
+            tree_info = sorted(rounds)
+        elif tree_info == "shuffled":
+            tree_info = [int(v) for v in rng.permutation(rounds)]
+        else:
+            raise ValueError(tree_info)
+    objective = "multi:softprob" if num_class else "binary:logistic"
+    return {"learner": {"objective": {"name": objective},
+                        "learner_model_param": {"base_score": repr(float(base_score)), "num_class": str(num_class),
+                                                "num_feature": str(x.shape[1])},
+                        "gradient_booster": {"name": "gbtree", "model": {"trees": trees, "tree_info": list(tree_info)}}}}
+
+
 def _expf(v: np.ndarray) -> np.ndarray:
     """libm's expf as xgboost's Sigmoid / Softmax call it: glibc's is correctly rounded for all but about one
     argument in 10^7, NumPy's SIMD float32 exp is not -- so: float64 exp, rounded once."""

@@ -96,28 +96,32 @@ void launch_k3(const DevPlan& plan, const float* feats, size_t row_stride, const
                uint8_t* low_score, float* probs, double* qual, double* phreds, int phred_mode, long long* d_counts, int,
                cudaStream_t) {
     one_thread_grid();
-    const size_t need = (size_t)plan.h.n_features * sizeof(float) + (size_t)plan.h.n_nodes * sizeof(uint2) +
+    // the product's forest buffer: a forest larger than it runs the chunk loop here too
+    const unsigned chunk = k3_infer_config(plan, 1).chunk;
+    const size_t need = (size_t)plan.h.n_features * sizeof(float) + (size_t)chunk * sizeof(uint2) +
                         ((size_t)plan.h.n_trees + 2) * sizeof(uint32_t);
     if (need > sizeof(smem3)) {
         fprintf(stderr, "host_emu: forest too large for the emulated shared memory\n");
         abort();
     }
-    k3_infer<1>(plan, feats, row_stride, d_n_records, threshold, low_score, probs, qual, phreds, d_counts,
-                plan.h.n_nodes, phred_mode);
+    k3_infer<1>(plan, feats, row_stride, d_n_records, threshold, low_score, probs, qual, phreds, d_counts, chunk,
+                phred_mode);
 }
 
 void launch_k3_fused(const DevPlan& plan, const uint32_t* raw, const float* feats, size_t row_stride,
                      const int64_t* d_n_records, double threshold, uint8_t* low_score, float* probs, double* qual,
                      double* phreds, int phred_mode, long long* d_counts, unsigned long long* d_err, int, cudaStream_t) {
     one_thread_grid();
+    // trees per staged chunk as the product's shape gives them: a forest larger than it runs the chunk loop here too
+    const unsigned chunk = k3_heap_config(plan, 1).chunk;
     const size_t need = (size_t)plan.h.n_features * (sizeof(float) + sizeof(PlanFeature)) + 64 +
-                        (size_t)plan.h.n_trees * ((size_t)10 << plan.heap_depth) + 64;
+                        (size_t)chunk * ((size_t)10 << plan.heap_depth) + 64;
     if (need > sizeof(smem3)) {
         fprintf(stderr, "host_emu: forest too large for the emulated shared memory\n");
         abort();
     }
     k3_heap<1, 1, 8, 1>(plan, raw, feats, row_stride, d_n_records, threshold, low_score, probs, qual, phreds, d_counts,
-               plan.h.n_trees, phred_mode, d_err);
+                        chunk, phred_mode, d_err);
 }
 
 cudaError_t kernels_configure(const DevPlan&) { return cudaSuccess; }

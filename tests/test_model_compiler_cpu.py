@@ -81,6 +81,52 @@ def test_xgboost_json_lowering():
     assert m["init"][0] == 0.0 and m["n_outputs"] == 1 and m["n_classes"] == 2
 
 
+def test_feature_and_class_limits_are_plan_errors():
+    """250 features and 4 classes are the plan's limits: one more of either is refused by every model kind, not
+    lowered into a plan the loader would refuse or mis-size."""
+    from sklearn.ensemble import GradientBoostingClassifier, RandomForestClassifier
+    from sklearn.linear_model import LogisticRegression
+
+    from oracle import xgb_predictor as XP
+
+    rng = np.random.default_rng(0)
+    x = rng.normal(size=(200, 251))
+    y2, y5 = (x[:, 0] > 0).astype(int), np.arange(200) % 5
+    with pytest.raises(MC.PlanError, match="feature count"):
+        MC.compile_plan_model_only(LogisticRegression(max_iter=50).fit(x, y2), 251)
+    assert MC.compile_plan_model_only(LogisticRegression(max_iter=50).fit(x[:, :250], y2), 250).n_features == 250
+    for model in (LogisticRegression(max_iter=50), GradientBoostingClassifier(n_estimators=2, max_depth=2),
+                  RandomForestClassifier(n_estimators=2, max_depth=2)):
+        with pytest.raises(MC.PlanError, match="too many classes"):
+            MC.compile_plan_model_only(model.fit(x[:, :5], y5), 5)
+    with pytest.raises(MC.PlanError, match="too many classes"):
+        MC.compile_plan_model_only(XP.random_gbtree_document(0, x[:, :5], 10, num_class=5, max_depth=3), 5)
+    assert MC.compile_plan_model_only(XP.random_gbtree_document(0, x[:, :5], 8, num_class=4, max_depth=3), 5).n_classes == 4
+
+
+def test_random_gbtree_documents():
+    """The seeded generator behind the deep xgboost tests: reproducible, unbalanced, the depths asked for."""
+    from oracle import xgb_predictor as XP
+
+    x = np.random.default_rng(1).normal(size=(50, 7)).astype(np.float32)
+    a = XP.random_gbtree_document(3, x, 40, num_class=3, max_depth=12, tree_info="shuffled")
+    assert a == XP.random_gbtree_document(3, x, 40, num_class=3, max_depth=12, tree_info="shuffled")
+    trees = a["learner"]["gradient_booster"]["model"]["trees"]
+
+    def depth(t, n=0):
+        return 0 if t["left_children"][n] == -1 else 1 + max(depth(t, t["left_children"][n]), depth(t, t["right_children"][n]))
+
+    depths = [depth(t) for t in trees]
+    assert max(depths) <= 12 and len(set(depths)) > 3
+    assert any(len(t["left_children"]) < 2 ** (depth(t) + 1) - 1 for t in trees)  # not complete trees
+    assert sorted(a["learner"]["gradient_booster"]["model"]["tree_info"]) == sorted(t % 3 for t in range(40))
+    conds = {np.float32(c) for t in trees for c, lc in zip(t["split_conditions"], t["left_children"]) if lc != -1}
+    assert conds <= set(x.ravel().tolist())
+    full = XP.random_gbtree_document(4, x, 5, max_depth=9, full_depth=True)
+    assert [depth(t) for t in full["learner"]["gradient_booster"]["model"]["trees"]] == [9] * 5
+    assert MC._lower_xgboost_json(full, 7)["n_trees"] == 5  # noqa: SLF001
+
+
 def test_no_model_plan():
     p = MC.compile_plan_no_model("##fileformat=VCFv4.2\n#CHROM\tPOS\n")
     assert p.n_features == 0 and len(p.blob) == 96

@@ -112,6 +112,15 @@ static int fail(ugvc_ctx* ctx, int code, const std::string& msg) {
             return fail(ctx, UGVC_E_CUDA, std::string(#call) + ": " + cudaGetErrorString(_e));     \
     } while (0)
 
+// UGVC_K3_LEGACY=1 (profiling): K2 + k3_infer even where k3_heap would run
+static bool k3_legacy() {
+    static const bool legacy = getenv("UGVC_K3_LEGACY") && *getenv("UGVC_K3_LEGACY") != '0';
+    return legacy;
+}
+// the K3 kernel of a plan with a model: k3_heap (K2 fused into its tile load) when the model has a heap form,
+// else K2 + k3_infer
+static bool k3_runs_heap(const DevPlan& p) { return !k3_legacy() && k3_fused_available(p); }
+
 extern "C" int ugvc_version(void) { return UGVC_VERSION; }
 
 extern "C" const char* ugvc_last_error(const ugvc_ctx* ctx) { return ctx ? ctx->err.c_str() : g_init_error.c_str(); }
@@ -621,14 +630,24 @@ extern "C" int ugvc_load_plan(ugvc_ctx* ctx, const void* blob, size_t n_bytes) {
     p.leaves = reinterpret_cast<const double*>(d + o_leaves);
     p.htab = ctx->d_htab;
     p.first_fixed_slot = first_fixed;
-    if (k1_smem_bytes(p) > 227 * 1024 || k3_smem_bytes(p) > 227 * 1024 || !k3_plan_fits(p))
-        return fail(ctx, UGVC_E_PLAN, "plan needs more shared memory than one sm_90 CTA has");
-    if (h.model_kind != MODEL_LOGISTIC && h.model_kind != MODEL_NONE) {
-        const uint32_t* root = reinterpret_cast<const uint32_t*>(hb + o_root);
-        const unsigned cap = k3_chunk_nodes_cap(p);
-        for (uint32_t t = 0; t < h.n_trees; ++t)
-            if (root[t + 1] - root[t] > cap)
-                return fail(ctx, UGVC_E_PLAN, "a single tree does not fit the shared-memory forest buffer");
+    if (k1_smem_bytes(p) > 227 * 1024)
+        return fail(ctx, UGVC_E_PLAN, "plan needs more shared memory than one sm_90 CTA has (K1 field parse)");
+    // the shared-memory limits are those of the K3 kernel that will run the model: k3_heap holds every plan the
+    // compiler makes (up to 250 features) when the model has a heap form, k3_infer fewer features
+    if (h.model_kind != MODEL_NONE && !k3_runs_heap(p)) {
+        if (k3_smem_bytes(p) > 227 * 1024 || !k3_plan_fits(p))
+            return fail(ctx, UGVC_E_PLAN,
+                        std::string("plan needs more shared memory than one sm_90 CTA has: k3_infer (") +
+                            (k3_legacy() ? "selected by UGVC_K3_LEGACY" : "forests deeper than 8 or with 65536 leaf rows or more") +
+                            ") holds at most " + std::to_string(k3_infer_max_features(p)) + " features for this model, it has " +
+                            std::to_string(h.n_features));
+        if (h.model_kind != MODEL_LOGISTIC) {
+            const uint32_t* root = reinterpret_cast<const uint32_t*>(hb + o_root);
+            const unsigned cap = k3_chunk_nodes_cap(p);
+            for (uint32_t t = 0; t < h.n_trees; ++t)
+                if (root[t + 1] - root[t] > cap)
+                    return fail(ctx, UGVC_E_PLAN, "a single tree does not fit k3_infer's shared-memory forest buffer");
+        }
     }
     CU(kernels_configure(p));
     ctx->h_tags.assign(tags, tags + h.n_tags);
@@ -859,8 +878,7 @@ static int enqueue_kernels(ugvc_ctx* ctx, Lane& l, const uint8_t* d_text, size_t
                   ctx->d_counts, ctx->sm_count, st);
     if (timing) CU(cudaEventRecord(ev[2], st));
     const bool has_model = p.h.model_kind != MODEL_NONE;
-    static const bool k3_legacy = getenv("UGVC_K3_LEGACY") && *getenv("UGVC_K3_LEGACY") != '0';  // profiling: K2 + preorder K3
-    const bool fused = has_model && !k3_legacy && k3_fused_available(p);
+    const bool fused = has_model && k3_runs_heap(p);
     if (has_model && !fused) launch_k2(p, l.b.raw, l.b.cap_records, d_n_records, l.b.feats, l.d_err, ctx->sm_count, st);
     if (timing) CU(cudaEventRecord(ev[3], st));
     if (fused)  // feature assembly happens in the tile load of the inference kernel
@@ -1405,7 +1423,7 @@ extern "C" int ugvc_predict_features(ugvc_ctx* ctx, const float* x, size_t n, si
                          cudaMemcpyHostToDevice, st));
     const int64_t n64 = (int64_t)n;
     CU(cudaMemcpyAsync(l.b.n_records, &n64, sizeof(n64), cudaMemcpyHostToDevice, st));
-    if (k3_fused_available(p))
+    if (k3_runs_heap(p))
         launch_k3_fused(p, nullptr, l.b.feats, l.b.cap_records, l.b.n_records, threshold, l.b.low_score, l.b.probs, l.b.qual,
                         l.b.phreds, ctx->want_phreds, ctx->d_counts, l.d_err, ctx->sm_count, st);
     else
@@ -1539,6 +1557,18 @@ extern "C" int ugvc_test_device_sigmoid(ugvc_ctx* ctx, const float* margins, int
 #else
 extern "C" int ugvc_test_device_sigmoid(ugvc_ctx*, const float*, int, float*, float*) { return UGVC_E_CUDA; }
 #endif
+
+extern "C" int ugvc_test_k3_config(ugvc_ctx* ctx, int32_t out[8]) {
+    // test hook: the K3 launch the loaded plan gets, from the functions the launchers use
+    if (!ctx || !out) return UGVC_E_ARG;
+    if (!ctx->has_plan || ctx->plan.h.model_kind == MODEL_NONE)
+        return fail(ctx, UGVC_E_STATE, "test_k3_config: load a plan with a model first");
+    const DevPlan& p = ctx->plan;
+    const K3Config c = k3_runs_heap(p) ? k3_heap_config(p, ctx->sm_count) : k3_infer_config(p, ctx->sm_count);
+    const int32_t v[8] = {c.kernel, c.tpb, c.nbuf, c.groups, c.nch, (int32_t)c.chunk, c.resident ? 1 : 0, c.grid};
+    memcpy(out, v, sizeof(v));
+    return UGVC_OK;
+}
 
 extern "C" int64_t ugvc_launch_count(const ugvc_ctx* ctx) { return ctx ? ctx->launches : 0; }
 

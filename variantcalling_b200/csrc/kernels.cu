@@ -1564,30 +1564,43 @@ bool k3_fused_available(const DevPlan& plan) {
     if (plan.h.model_kind != MODEL_LOGISTIC && plan.heap_depth == 0) return false;
     return k3h_shape(plan).tpb != 0;
 }
+K3Config k3_heap_config(const DevPlan& plan, int sm_count) {
+    const K3hShape sh = k3h_shape(plan);
+    K3Config c{};
+    c.kernel = K3_KERNEL_HEAP;
+    c.tpb = sh.tpb;
+    c.nbuf = sh.nbuf;
+    c.groups = sh.groups;
+    // few threads per SM (the tiles are large): sixteen trees per thread in flight make up for it
+    static const int nch448 = getenv("UGVC_K3_NCH448") ? atoi(getenv("UGVC_K3_NCH448")) : 8;  // profiling knob
+    if (sh.groups == 2) c.nch = sh.tpb == 512 ? 8 : sh.tpb == 448 ? (nch448 == 12 ? 12 : 8) : 16;
+    else c.nch = sh.nbuf == 2 ? 16 : 8;
+    c.chunk = k3h_chunk_trees(plan, sh);
+    c.resident = plan.h.model_kind == MODEL_LOGISTIC || c.chunk >= plan.h.n_trees;
+    c.smem = k3h_tile_bytes(plan, sh) + (size_t)c.chunk * k3h_tree_bytes(plan);
+    int per_sm = (int)((227u * 1024u) / (c.smem + 1024));
+    per_sm = per_sm < 1 ? 1 : (per_sm > 4 ? 4 : per_sm);
+    if (per_sm * sh.tpb > 1536) per_sm = 1536 / sh.tpb;
+    c.grid = sm_count * per_sm;
+    return c;
+}
 #ifndef UGVC_HOST_EMU
 void launch_k3_fused(const DevPlan& plan, const uint32_t* raw, const float* feats, size_t row_stride,
                      const int64_t* d_n_records, double threshold, uint8_t* low_score, float* probs, double* qual,
                      double* phreds, int phred_mode, long long* d_counts, unsigned long long* d_err, int sm_count,
                      cudaStream_t st) {
-    const K3hShape sh = k3h_shape(plan);
-    const unsigned chunk = k3h_chunk_trees(plan, sh);
-    const size_t smem = k3h_tile_bytes(plan, sh) + (size_t)chunk * k3h_tree_bytes(plan);
-    int per_sm = (int)((227u * 1024u) / (smem + 1024));
-    per_sm = per_sm < 1 ? 1 : (per_sm > 4 ? 4 : per_sm);
-    if (per_sm * sh.tpb > 1536) per_sm = 1536 / sh.tpb;
-    // few threads per SM (the tiles are large): sixteen trees per thread in flight make up for it
+    const K3Config c = k3_heap_config(plan, sm_count);
 #define K3H_LAUNCH(T, B, C, G)                                                                                                  \
-    k3_heap<T, B, C, G><<<sm_count * per_sm, T, smem, st>>>(plan, raw, feats, row_stride, d_n_records, threshold, low_score, probs, \
-                                                            qual, phreds, d_counts, chunk, phred_mode, d_err)
-    static const int nch448 = getenv("UGVC_K3_NCH448") ? atoi(getenv("UGVC_K3_NCH448")) : 8;  // profiling knob
-    if (sh.groups == 2 && sh.tpb == 512) K3H_LAUNCH(512, 1, 8, 2);
-    else if (sh.groups == 2 && sh.tpb == 448 && nch448 == 12) K3H_LAUNCH(448, 1, 12, 2);
-    else if (sh.groups == 2 && sh.tpb == 448) K3H_LAUNCH(448, 1, 8, 2);
-    else if (sh.groups == 2) K3H_LAUNCH(384, 1, 16, 2);
-    else if (sh.tpb == 256 && sh.nbuf == 2) K3H_LAUNCH(256, 2, 16, 1);
-    else if (sh.tpb == 192) K3H_LAUNCH(192, 2, 16, 1);
-    else if (sh.tpb == 256) K3H_LAUNCH(256, 1, 8, 1);
-    else if (sh.nbuf == 2) K3H_LAUNCH(128, 2, 16, 1);
+    k3_heap<T, B, C, G><<<c.grid, T, c.smem, st>>>(plan, raw, feats, row_stride, d_n_records, threshold, low_score, probs, \
+                                                   qual, phreds, d_counts, c.chunk, phred_mode, d_err)
+    if (c.groups == 2 && c.tpb == 512) K3H_LAUNCH(512, 1, 8, 2);
+    else if (c.groups == 2 && c.tpb == 448 && c.nch == 12) K3H_LAUNCH(448, 1, 12, 2);
+    else if (c.groups == 2 && c.tpb == 448) K3H_LAUNCH(448, 1, 8, 2);
+    else if (c.groups == 2) K3H_LAUNCH(384, 1, 16, 2);
+    else if (c.tpb == 256 && c.nbuf == 2) K3H_LAUNCH(256, 2, 16, 1);
+    else if (c.tpb == 192) K3H_LAUNCH(192, 2, 16, 1);
+    else if (c.tpb == 256) K3H_LAUNCH(256, 1, 8, 1);
+    else if (c.nbuf == 2) K3H_LAUNCH(128, 2, 16, 1);
     else K3H_LAUNCH(128, 1, 8, 1);
 #undef K3H_LAUNCH
 }
@@ -1626,21 +1639,38 @@ bool k3_plan_fits(const DevPlan& plan) {
     if (k3_forest_bytes(plan) == 0) return (size_t)plan.h.n_features * 256 * sizeof(float) <= K3_SMEM_BUDGET;
     return k3_chunk_nodes(plan) > 0;
 }
+// most features k3_infer holds for this model: a 256-record tile, plus for a forest the tree roots and 4 KiB of nodes
+unsigned k3_infer_max_features(const DevPlan& plan) {
+    const size_t fixed = k3_forest_bytes(plan) ? k3_roots_bytes(plan) + 4096 : 0;
+    return fixed >= K3_SMEM_BUDGET ? 0u : (unsigned)((K3_SMEM_BUDGET - fixed) / (256 * sizeof(float)));
+}
+K3Config k3_infer_config(const DevPlan& plan, int sm_count) {
+    K3Config c{};
+    c.kernel = K3_KERNEL_INFER;
+    c.tpb = k3_tpb(plan);
+    c.nbuf = c.groups = 1;
+    c.nch = K3_CHAINS;
+    c.chunk = k3_chunk_nodes(plan);
+    c.resident = k3_forest_bytes(plan) == 0 || c.chunk >= plan.h.n_nodes;
+    c.smem = k3_smem_bytes(plan);
+    int per_sm = (int)((K3_SMEM_BUDGET) / (c.smem + 1024));
+    if (per_sm < 1) per_sm = 1;
+    if (per_sm > 4) per_sm = 4;
+    c.grid = sm_count * per_sm;
+    return c;
+}
 
 #ifndef UGVC_HOST_EMU
 void launch_k3(const DevPlan& plan, const float* feats, size_t row_stride, const int64_t* d_n_records,
                double threshold, uint8_t* low_score, float* probs, double* qual, double* phreds, int phred_mode,
                long long* d_counts, int sm_count, cudaStream_t st) {
-    const size_t smem = k3_smem_bytes(plan);
-    int per_sm = (int)((K3_SMEM_BUDGET) / (smem + 1024));
-    if (per_sm < 1) per_sm = 1;
-    if (per_sm > 4) per_sm = 4;
-    if (k3_tpb(plan) == 384)
-        k3_infer<384><<<sm_count * per_sm, 384, smem, st>>>(plan, feats, row_stride, d_n_records, threshold, low_score,
-                                                            probs, qual, phreds, d_counts, k3_chunk_nodes(plan), phred_mode);
+    const K3Config c = k3_infer_config(plan, sm_count);
+    if (c.tpb == 384)
+        k3_infer<384><<<c.grid, 384, c.smem, st>>>(plan, feats, row_stride, d_n_records, threshold, low_score,
+                                                   probs, qual, phreds, d_counts, c.chunk, phred_mode);
     else
-        k3_infer<256><<<sm_count * per_sm, 256, smem, st>>>(plan, feats, row_stride, d_n_records, threshold, low_score,
-                                                            probs, qual, phreds, d_counts, k3_chunk_nodes(plan), phred_mode);
+        k3_infer<256><<<c.grid, 256, c.smem, st>>>(plan, feats, row_stride, d_n_records, threshold, low_score,
+                                                   probs, qual, phreds, d_counts, c.chunk, phred_mode);
 }
 
 cudaError_t kernels_configure(const DevPlan& plan) {

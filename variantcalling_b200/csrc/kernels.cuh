@@ -185,8 +185,22 @@ void launch_k1_fast(const DevPlan& plan, const DevFast& fast, const DevSchedule&
                     uint32_t* scratch, int64_t* line_start, size_t cap_records, int64_t* d_n_records, uint32_t* raw,
                     size_t row_stride, ugvc_recinfo* recinfo, uint32_t* slow_list, unsigned long long* d_err,
                     long long* d_counts, int sm_count, cudaStream_t st);
+// The K3 launch of a plan, as launch_k3_fused (k3_heap) / launch_k3 (k3_infer) make it; ugvc_test_k3_config reports it
+enum { K3_KERNEL_HEAP = 0, K3_KERNEL_INFER = 1 };
+struct K3Config {
+    int kernel;             // K3_KERNEL_HEAP / K3_KERNEL_INFER
+    int tpb, nbuf, groups;  // threads per CTA, tile buffers per group, independent groups per CTA (records per tile: tpb / groups)
+    int nch;                // trees one thread walks at once
+    unsigned chunk;         // k3_heap: trees per staged forest chunk; k3_infer: nodes the forest buffer holds (0: linear model)
+    bool resident;          // the whole model is staged once (no chunk loop)
+    size_t smem;            // dynamic shared memory per CTA
+    int grid;               // CTAs of the persistent grid
+};
+K3Config k3_heap_config(const DevPlan& plan, int sm_count);   // only when k3_fused_available(plan)
+K3Config k3_infer_config(const DevPlan& plan, int sm_count);
 size_t k1_smem_bytes(const DevPlan& plan);
 size_t k3_smem_bytes(const DevPlan& plan);
 bool k3_plan_fits(const DevPlan& plan);
 unsigned k3_chunk_nodes_cap(const DevPlan& plan);
+unsigned k3_infer_max_features(const DevPlan& plan);
 cudaError_t kernels_configure(const DevPlan& plan);

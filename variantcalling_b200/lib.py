@@ -111,6 +111,7 @@ SIGNATURES = {
     "ugvc_test_deflate_block": (C.c_int64, [_vp, C.c_uint32, _vp]),
     "ugvc_test_deflate_block_lanes": (C.c_int64, [_vp, C.c_uint32, _vp]),
     "ugvc_test_device_sigmoid": (C.c_int, [_vp, _vp, C.c_int, _vp, _vp]),
+    "ugvc_test_k3_config": (C.c_int, [_vp, _vp]),
     "ugvc_bgzf_range_info": (C.c_int, [C.c_char_p, C.c_uint64, C.c_uint64, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64),
                                        C.POINTER(C.c_uint32), C.POINTER(C.c_uint64)]),
     "ugvc_filter_bgzf": (C.c_int, [_vp, C.c_int, _vp, _sz, C.c_uint32, C.c_uint64, C.c_double, C.c_int, _vp, _sz, C.POINTER(_sz),
@@ -419,6 +420,14 @@ class Context:
 
     def launch_count(self) -> int:
         return int(self.lib.ugvc_launch_count(self.h))
+
+    def k3_config(self) -> dict:
+        """The K3 launch the loaded plan gets (test hook ugvc_test_k3_config)."""
+        out = np.zeros(8, np.int32)
+        self._check(self.lib.ugvc_test_k3_config(self.h, _ptr(out)))
+        kernel, tpb, nbuf, groups, nch, chunk, resident, grid = (int(v) for v in out)
+        return {"kernel": ("heap", "infer")[kernel], "tpb": tpb, "nbuf": nbuf, "groups": groups, "nch": nch, "chunk": chunk,
+                "resident": bool(resident), "grid": grid, "gs": tpb // groups}
 
     def enable_stage_timing(self, on: bool = True):
         self._check(self.lib.ugvc_enable_stage_timing(self.h, int(on)))

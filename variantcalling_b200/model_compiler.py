@@ -409,6 +409,8 @@ def _lower_model(model, n_features: int) -> dict:  # noqa: C901, PLR0912, PLR091
                     n_trees=0, n_nodes=0, n_leaf_rows=0, leaf_width=0, classes=list(model.classes_))
     if cls == "GradientBoostingClassifier":
         k = len(model.classes_)
+        if k > MAX_CLASSES:
+            raise PlanError("too many classes")
         est = model.estimators_
         n_out = est.shape[1]
         if getattr(model, "n_features_in_", n_features) != n_features:
