@@ -141,7 +141,9 @@ int ugvc_bgzf_inflate_device(ugvc_ctx* ctx, const uint8_t* bgzf, size_t n_bytes,
  * n_features columns are the features of a plan compiled with model_compiler.compile_plan_model_only
  * (or any plan with a model).  n <= the max_records of ugvc_reserve; outputs may be NULL; with
  * ugvc_enable_phreds(ctx, 2) the fp64 class probabilities are fetched with ugvc_collect_phreds(ctx, 0, ...).
- * A NaN / infinite input value is UGVC_E_DATA (the reference's estimators raise on it). */
+ * An infinite input value is UGVC_E_DATA, and so is NaN unless the plan's model is xgboost (the reference's sklearn
+ * estimators raise on it).  For an xgboost model NaN is a missing value: every node sends it to its default child
+ * (default_left), as xgboost's predictor does; the row and column of a refused value come from ugvc_last_data_error. */
 int ugvc_predict_features(ugvc_ctx* ctx, const float* x, size_t n, size_t ld, double threshold,
                           uint8_t* out_low_score, float* out_probs, double* out_qual);
 
@@ -383,8 +385,9 @@ int ugvc_test_device_sigmoid(ugvc_ctx* ctx, const float* margins, int n, float* 
 /* Test hook: the K3 launch the loaded plan gets (also in the host emulation, which runs the same chunking).
  * out = {kernel (0 k3_heap, 1 k3_infer), threads per CTA, tile buffers per group, groups per CTA (records per tile:
  * threads / groups), trees one thread walks at once, forest chunk (k3_heap: trees, k3_infer: nodes; 0 for a linear
- * model), 1 when the whole model is staged once, CTAs of the persistent grid}.  UGVC_E_STATE without a model. */
-int ugvc_test_k3_config(ugvc_ctx* ctx, int32_t out[8]);
+ * model), 1 when the whole model is staged once, CTAs of the persistent grid, tree walk (0 plain; 1 default-left /
+ * categorical routing of an xgboost model with such nodes)}.  UGVC_E_STATE without a model. */
+int ugvc_test_k3_config(ugvc_ctx* ctx, int32_t out[9]);
 int ugvc_test_parse_float(const char* text, float* out_f32, double* out_f64, int* out_consumed);
 /* Test hook: the device BGZF encoder (csrc/deflate.cuh) run on the host on one block of at most 57344 bytes (4 readable
  * bytes after n); out receives a complete BGZF block (<= 65536 bytes), the size is returned. */

@@ -412,7 +412,8 @@ extern "C" int ugvc_load_plan(ugvc_ctx* ctx, const void* blob, size_t n_bytes) {
     off = align8(off + (size_t)h.n_checks * sizeof(PlanCheck));
     const size_t o_combines = off;
     off = align8(off + (size_t)h.n_combines * sizeof(PlanCombine));
-    size_t o_coef = 0, o_icpt = 0, o_root = 0, o_tout = 0, o_nodes = 0, o_leaves = 0;
+    size_t o_coef = 0, o_icpt = 0, o_root = 0, o_tout = 0, o_nodes = 0, o_leaves = 0, o_flags = 0, o_cat = 0;
+    PlanCatHeader cat_h{0, 0};
     if (h.model_kind == MODEL_LOGISTIC) {
         o_coef = off;
         off = align8(off + (size_t)h.n_outputs * h.n_features * sizeof(double));
@@ -427,6 +428,14 @@ extern "C" int ugvc_load_plan(ugvc_ctx* ctx, const void* blob, size_t n_bytes) {
         off = align8(off + (size_t)h.n_nodes * sizeof(PlanNode));
         o_leaves = off;
         off = align8(off + (size_t)h.n_leaf_rows * h.leaf_width * sizeof(double));
+        o_flags = off;
+        off = align8(off + (size_t)h.n_nodes);
+        if (off + sizeof(PlanCatHeader) > n_bytes) return fail(ctx, UGVC_E_PLAN, "plan blob truncated");
+        memcpy(&cat_h, static_cast<const uint8_t*>(blob) + off, sizeof(cat_h));
+        off += sizeof(PlanCatHeader);
+        if (cat_h.n_words >= (1u << 24)) return fail(ctx, UGVC_E_PLAN, "too many category bitset words");
+        o_cat = off;
+        off = align8(off + (size_t)cat_h.n_words * sizeof(uint32_t));
     } else if (h.model_kind == MODEL_NONE) {
         if (h.n_features != 0) return fail(ctx, UGVC_E_PLAN, "a plan without a model cannot have features");
     } else {
@@ -474,23 +483,40 @@ extern "C" int ugvc_load_plan(ugvc_ctx* ctx, const void* blob, size_t n_bytes) {
         const uint32_t* root = reinterpret_cast<const uint32_t*>(hb + o_root);
         const PlanNode* nodes = reinterpret_cast<const PlanNode*>(hb + o_nodes);
         const uint8_t* tout = hb + o_tout;
+        const uint8_t* nflags = hb + o_flags;
+        uint32_t n_flagged = 0;
         for (uint32_t t = 0; t < h.n_trees; ++t) {
             if (root[t] > root[t + 1] || root[t + 1] > h.n_nodes) return fail(ctx, UGVC_E_PLAN, "tree roots not monotone");
             if (tout[t] >= h.n_outputs) return fail(ctx, UGVC_E_PLAN, "tree output out of range");
             const uint32_t n = root[t + 1] - root[t];
             for (uint32_t i = 0; i < n; ++i) {
                 const PlanNode& nd = nodes[root[t] + i];
+                const uint8_t fl = nflags[root[t] + i];
+                if (fl & ~(NODE_DEFAULT_LEFT | NODE_CATEGORICAL)) return fail(ctx, UGVC_E_PLAN, "unknown node flag");
+                if (fl && h.model_kind != MODEL_XGB) return fail(ctx, UGVC_E_PLAN, "node flags on a model other than xgboost");
+                n_flagged += fl ? 1u : 0u;
                 if (nd.feature >= 0) {
                     if ((uint32_t)nd.feature >= h.n_features || nd.right >= n || i + 1 >= n)
                         return fail(ctx, UGVC_E_PLAN, "tree node out of range");
+                    if (fl & NODE_CATEGORICAL) {  // the node's bitset lies inside the category section
+                        uint32_t ref;
+                        memcpy(&ref, &nd.value, 4);
+                        const uint32_t words = UGVC_CAT_WORDS(ref);
+                        if (words == 0 || words > UGVC_CAT_MAX_WORDS || UGVC_CAT_FIRST(ref) + words > cat_h.n_words)
+                            return fail(ctx, UGVC_E_PLAN, "category bitset reference out of range");
+                    }
                 } else {
+                    if (fl) return fail(ctx, UGVC_E_PLAN, "node flags on a leaf");
                     int32_t leaf;
                     memcpy(&leaf, &nd.value, 4);
                     if (leaf < 0 || (uint32_t)leaf >= h.n_leaf_rows) return fail(ctx, UGVC_E_PLAN, "leaf row out of range");
                 }
             }
         }
+        if (n_flagged != cat_h.n_flagged) return fail(ctx, UGVC_E_PLAN, "flagged node count does not match the node flags");
     }
+    // walk variant, chosen once here: the plain walks unless a node routes by a flag
+    const uint32_t walk = cat_h.n_flagged ? K3_WALK_CAT : K3_WALK_PLAIN;
     // device form of the forest: leaves become absorbing nodes (threshold = quiet NaN carrying the
     // leaf row, right child = itself) so a fixed-depth, branch-free walk ends on them; right
     // children are absolute indices.  Also the depth of the deepest leaf.
@@ -499,9 +525,14 @@ extern "C" int ugvc_load_plan(ugvc_ctx* ctx, const void* blob, size_t n_bytes) {
     if (h.model_kind != MODEL_LOGISTIC && h.model_kind != MODEL_NONE) {
         const uint32_t* root = reinterpret_cast<const uint32_t*>(hb + o_root);
         const PlanNode* nodes = reinterpret_cast<const PlanNode*>(hb + o_nodes);
-        if (h.n_nodes >= (1u << 24) || h.n_leaf_rows >= (1u << 22) || h.n_features > 255)
+        const uint8_t* nflags = hb + o_flags;
+        // the categorical walk keeps the node flags in bits 8-9 of y: right children take 22 bits there
+        const unsigned rsh = walk == K3_WALK_CAT ? 10u : 8u;
+        if (h.n_nodes >= (1u << (32 - rsh)) || h.n_leaf_rows >= (1u << 22) || h.n_features > 255)
             return fail(ctx, UGVC_E_PLAN, "forest too large for the device node format");
-        dev_nodes.resize(h.n_nodes);
+        // the category bitset words follow the nodes in the same device allocation
+        dev_nodes.resize(h.n_nodes + (cat_h.n_words + 1) / 2);
+        if (cat_h.n_words) memcpy(dev_nodes.data() + h.n_nodes, hb + o_cat, (size_t)cat_h.n_words * sizeof(uint32_t));
         std::vector<uint32_t> depth(h.n_nodes, 0);
         for (uint32_t t = 0; t < h.n_trees; ++t) {
             const uint32_t r0 = root[t], n = root[t + 1] - root[t];
@@ -511,13 +542,13 @@ extern "C" int ugvc_load_plan(ugvc_ctx* ctx, const void* blob, size_t n_bytes) {
                 if (nd.feature >= 0) {
                     uint32_t thr;
                     memcpy(&thr, &nd.value, 4);
-                    dev_nodes[r0 + i] = make_uint2(thr, (uint32_t)nd.feature | ((r0 + nd.right) << 8));
+                    dev_nodes[r0 + i] = make_uint2(thr, (uint32_t)nd.feature | ((uint32_t)nflags[r0 + i] << 8) | ((r0 + nd.right) << rsh));
                     depth[r0 + i + 1] = depth[r0 + i] + 1;
                     depth[r0 + nd.right] = depth[r0 + i] + 1;
                 } else {
                     int32_t leaf;
                     memcpy(&leaf, &nd.value, 4);
-                    dev_nodes[r0 + i] = make_uint2(0x7FC00000u | (uint32_t)leaf, (r0 + i) << 8);
+                    dev_nodes[r0 + i] = make_uint2(0x7FC00000u | (uint32_t)leaf, (r0 + i) << rsh);
                     if (depth[r0 + i] > max_depth) max_depth = depth[r0 + i];
                 }
             }
@@ -525,7 +556,9 @@ extern "C" int ugvc_load_plan(ugvc_ctx* ctx, const void* blob, size_t n_bytes) {
     }
 
     // heap form for k3_heap: every tree padded to a complete binary tree (breadth-first, root at index 1);
-    // below a shallow leaf every node is (+inf, feature 0) and every leaf slot carries its row
+    // below a shallow leaf every node is (+inf, feature 0, no flags) and every leaf slot carries its row, so a row
+    // reaches it whichever way it goes there (NaN included).  The categorical walk's node flags follow the features
+    // in the same array (heap_feat[n_trees * H + i]); a categorical node's threshold word is its bitset reference.
     std::vector<float> heap_thr;
     std::vector<uint8_t> heap_feat;
     std::vector<uint16_t> heap_leaf;
@@ -537,7 +570,8 @@ extern "C" int ugvc_load_plan(ugvc_ctx* ctx, const void* blob, size_t n_bytes) {
         const uint32_t H = 1u << heap_depth;
         const float inf = __builtin_huge_valf();
         heap_thr.assign((size_t)h.n_trees * H, inf);
-        heap_feat.assign((size_t)h.n_trees * H, 0);
+        heap_feat.assign((size_t)h.n_trees * H * (walk == K3_WALK_CAT ? 2 : 1), 0);
+        const uint8_t* nflags = hb + o_flags;
         heap_leaf.assign((size_t)h.n_trees * H, 0);
         struct Item { uint32_t node, heap, level; int32_t leaf; };  // leaf >= 0: inside a padded subtree
         std::vector<Item> stack;
@@ -557,6 +591,7 @@ extern "C" int ugvc_load_plan(ugvc_ctx* ctx, const void* blob, size_t n_bytes) {
                     if (nd.feature >= 0) {
                         thr[it.heap] = nd.value;
                         ft[it.heap] = (uint8_t)nd.feature;
+                        if (walk == K3_WALK_CAT) ft[(size_t)h.n_trees * H + it.heap] = nflags[r0 + it.node];
                         stack.push_back({it.node + 1, 2 * it.heap, it.level + 1, -1});
                         stack.push_back({nd.right, 2 * it.heap + 1, it.level + 1, -1});
                         continue;
@@ -623,6 +658,8 @@ extern "C" int ugvc_load_plan(ugvc_ctx* ctx, const void* blob, size_t n_bytes) {
     p.nodes = reinterpret_cast<const PlanNode*>(d + o_nodes);
     p.dev_nodes = ctx->d_nodes;
     p.max_depth = max_depth;
+    p.walk = walk;
+    p.n_cat_words = cat_h.n_words;
     p.heap_thr = ctx->d_heap_thr;
     p.heap_feat = ctx->d_heap_feat;
     p.heap_leaf = ctx->d_heap_leaf;
@@ -1400,15 +1437,16 @@ extern "C" int ugvc_predict_features(ugvc_ctx* ctx, const float* x, size_t n, si
     CU(cudaSetDevice(ctx->device));
     l.last_n = (int64_t)n;
     if (n == 0) return UGVC_OK;
-    // feature-major staging copy; a non-finite value is refused like the reference's estimators do
-    // ("Input X contains NaN / infinity"; xgboost's missing-value routing is not part of this path)
+    // feature-major staging copy; +-inf is refused like the reference's estimators do ("Input X contains NaN /
+    // infinity"), NaN too unless the model is xgboost's: there it is a missing value that K3 sends to the default child
+    const bool nan_ok = p.h.model_kind == MODEL_XGB;
     std::vector<float> cols(F * n);
     for (size_t r0 = 0; r0 < n; r0 += 256) {
         const size_t r1 = r0 + 256 < n ? r0 + 256 : n;
         for (size_t f = 0; f < F; ++f)
             for (size_t r = r0; r < r1; ++r) {
                 const float v = x[r * ld + f];
-                if (!(v - v == 0.0f)) {  // NaN or +-inf
+                if (!(v - v == 0.0f) && !(nan_ok && v != v)) {  // +-inf, or NaN where it is not a missing value
                     ctx->err_record = (int64_t)r;
                     ctx->err_column = (int32_t)f;
                     ctx->err_reason = REASON_NULL_FEATURE;
@@ -1558,14 +1596,14 @@ extern "C" int ugvc_test_device_sigmoid(ugvc_ctx* ctx, const float* margins, int
 extern "C" int ugvc_test_device_sigmoid(ugvc_ctx*, const float*, int, float*, float*) { return UGVC_E_CUDA; }
 #endif
 
-extern "C" int ugvc_test_k3_config(ugvc_ctx* ctx, int32_t out[8]) {
+extern "C" int ugvc_test_k3_config(ugvc_ctx* ctx, int32_t out[9]) {
     // test hook: the K3 launch the loaded plan gets, from the functions the launchers use
     if (!ctx || !out) return UGVC_E_ARG;
     if (!ctx->has_plan || ctx->plan.h.model_kind == MODEL_NONE)
         return fail(ctx, UGVC_E_STATE, "test_k3_config: load a plan with a model first");
     const DevPlan& p = ctx->plan;
     const K3Config c = k3_runs_heap(p) ? k3_heap_config(p, ctx->sm_count) : k3_infer_config(p, ctx->sm_count);
-    const int32_t v[8] = {c.kernel, c.tpb, c.nbuf, c.groups, c.nch, (int32_t)c.chunk, c.resident ? 1 : 0, c.grid};
+    const int32_t v[9] = {c.kernel, c.tpb, c.nbuf, c.groups, c.nch, (int32_t)c.chunk, c.resident ? 1 : 0, c.grid, c.walk};
     memcpy(out, v, sizeof(v));
     return UGVC_OK;
 }

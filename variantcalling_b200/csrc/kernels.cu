@@ -998,6 +998,46 @@ __device__ __forceinline__ void walk8(const uint2* __restrict__ s_nodes, const u
     for (int j = 0; j < K3_CHAINS; ++j) leaf[j] = (int)(nd[j].x & 0x3FFFFFu);
 }
 
+// K3_WALK_CAT: one node's decision (xgboost's GetNextNode / common::Decision, plan.h NODE_*).  NaN takes the default
+// child; a categorical node sends a category in its set right and everything else left (not in the set, past the
+// bitset, x < 0 or x >= 2^24); a numeric node goes left when x < threshold.  `word` is the threshold bits or the
+// node's UGVC_CAT_REF; s_cat the category bitset words in shared memory.
+__device__ __forceinline__ bool k3_cat_left(float xv, uint32_t word, uint32_t flags, const uint32_t* __restrict__ s_cat) {
+    const bool cat = (flags & NODE_CATEGORICAL) != 0;
+    const bool valid = xv >= 0.0f && xv < 16777216.0f;  // false for NaN too
+    const unsigned c = valid ? (unsigned)xv : 0u;         // truncation, as xgboost's AsCat
+    const bool in_bits = cat && valid && c < UGVC_CAT_WORDS(word) * 32u;
+    const bool in_set = in_bits && ((s_cat[UGVC_CAT_FIRST(word) + (c >> 5)] >> (c & 31u)) & 1u) != 0u;
+    const bool by_value = cat ? !in_set : xv < __uint_as_float(word);
+    return isnan(xv) ? (flags & NODE_DEFAULT_LEFT) != 0 : by_value;
+}
+
+// walk8 for K3_WALK_CAT plans (xgboost, so x < threshold): y = feature | flags << 8 | right << 10
+template <int TPB>
+__device__ __forceinline__ void walk8c(const uint2* __restrict__ s_nodes, const uint32_t* __restrict__ s_roots,
+                                       const uint32_t* __restrict__ s_cat, unsigned chunk_first_node, unsigned tr,
+                                       unsigned tr_end, int depth, const float* __restrict__ x, int leaf[K3_CHAINS]) {
+    unsigned n[K3_CHAINS];
+    uint2 nd[K3_CHAINS];
+#pragma unroll
+    for (int j = 0; j < K3_CHAINS; ++j) {
+        const unsigned t = tr + j < tr_end ? tr + j : tr;  // pad with a repeat (result ignored)
+        n[j] = s_roots[t] - chunk_first_node;
+    }
+    for (int d = 0; d <= depth; ++d) {
+#pragma unroll
+        for (int j = 0; j < K3_CHAINS; ++j) nd[j] = s_nodes[n[j]];
+#pragma unroll
+        for (int j = 0; j < K3_CHAINS; ++j) {
+            const float xv = x[(nd[j].y & 0xFFu) * TPB];
+            const bool left = k3_cat_left(xv, nd[j].x, (nd[j].y >> 8) & 3u, s_cat);  // false on a leaf (NaN, no flags)
+            n[j] = left ? n[j] + 1 : (nd[j].y >> 10) - chunk_first_node;
+        }
+    }
+#pragma unroll
+    for (int j = 0; j < K3_CHAINS; ++j) leaf[j] = (int)(nd[j].x & 0x3FFFFFu);
+}
+
 #ifndef UGVC_HOST_EMU
 // test hook: the xgboost-flavoured fp32 sigmoid exactly as k3_finish evaluates it, on an array of margins
 __global__ void k3_test_sigmoid(const float* __restrict__ m, int n, float* __restrict__ p1, float* __restrict__ e_out) {
@@ -1137,14 +1177,13 @@ __device__ __forceinline__ bool k3_finish(const DevPlan& plan, const float* __re
     return low;
 }
 
-template <int TPB>
-__global__ void __launch_bounds__(TPB, 1) k3_infer(const __grid_constant__ DevPlan plan,
-                                                      const float* __restrict__ feats, size_t row_stride,
-                                                      const int64_t* __restrict__ n_records_p, double threshold,
-                                                      uint8_t* __restrict__ low_score, float* __restrict__ probs,
-                                                      double* __restrict__ qual_out, double* __restrict__ phred_out,
-                                                      long long* counts, unsigned chunk_nodes_cap,
-                                                      int phred_mode) {
+// k3_infer's body; WALK: K3_WALK_* (one kernel per walk, chosen by the launcher from plan.walk)
+template <int TPB, int WALK>
+__device__ __forceinline__ void k3_infer_run(const DevPlan& plan, const float* __restrict__ feats, size_t row_stride,
+                                             const int64_t* __restrict__ n_records_p, double threshold,
+                                             uint8_t* __restrict__ low_score, float* __restrict__ probs,
+                                             double* __restrict__ qual_out, double* __restrict__ phred_out,
+                                             long long* counts, unsigned chunk_nodes_cap, int phred_mode) {
     extern __shared__ __align__(16) uint8_t smem3[];
     const int F = plan.h.n_features, K = plan.h.n_classes, O = plan.h.n_outputs;
     const unsigned n_trees = plan.h.n_trees;
@@ -1152,9 +1191,14 @@ __global__ void __launch_bounds__(TPB, 1) k3_infer(const __grid_constant__ DevPl
     float* tile = reinterpret_cast<float*>(smem3);  // [F][TPB]
     uint2* s_nodes = reinterpret_cast<uint2*>(smem3 + (size_t)F * TPB * sizeof(float));
     uint32_t* s_roots = reinterpret_cast<uint32_t*>(s_nodes + chunk_nodes_cap);  // [n_trees + 1]
+    uint32_t* s_cat = s_roots + n_trees + 2;                                      // [n_cat_words], always resident
     const bool resident = forest && plan.h.n_nodes <= chunk_nodes_cap;  // whole forest fits: stage once
     if (forest) {
         for (unsigned i = threadIdx.x; i <= n_trees; i += TPB) s_roots[i] = plan.tree_root[i];
+        if (WALK == K3_WALK_CAT) {
+            const uint32_t* cat = reinterpret_cast<const uint32_t*>(plan.dev_nodes + plan.h.n_nodes);
+            for (unsigned i = threadIdx.x; i < plan.n_cat_words; i += TPB) s_cat[i] = cat[i];
+        }
         if (resident)
             for (unsigned i = threadIdx.x; i < plan.h.n_nodes; i += TPB) s_nodes[i] = plan.dev_nodes[i];
     }
@@ -1198,7 +1242,8 @@ __global__ void __launch_bounds__(TPB, 1) k3_infer(const __grid_constant__ DevPl
                 }
                 for (unsigned tr = c0; tr < c1; tr += K3_CHAINS) {
                     int leaf[K3_CHAINS];
-                    if (plan.h.cmp_mode == CMP_LE) walk8<CMP_LE, TPB>(s_nodes, s_roots, first_node, tr, c1, depth, x, leaf);
+                    if (WALK == K3_WALK_CAT) walk8c<TPB>(s_nodes, s_roots, s_cat, first_node, tr, c1, depth, x, leaf);
+                    else if (plan.h.cmp_mode == CMP_LE) walk8<CMP_LE, TPB>(s_nodes, s_roots, first_node, tr, c1, depth, x, leaf);
                     else walk8<CMP_LT, TPB>(s_nodes, s_roots, first_node, tr, c1, depth, x, leaf);
                     if (plan.h.model_kind == MODEL_GB_SKLEARN && O == 1) {
                         // raw += learning_rate * leaf (pre-scaled on the host), fp64, tree order
@@ -1250,6 +1295,28 @@ __global__ void __launch_bounds__(TPB, 1) k3_infer(const __grid_constant__ DevPl
         atomicAdd((unsigned long long*)&counts[2], (unsigned long long)(n_seen - n_low));
     }
 }
+
+#define K3_INFER_PARAMS                                                                                                 \
+    const __grid_constant__ DevPlan plan, const float* __restrict__ feats, size_t row_stride,                           \
+        const int64_t* __restrict__ n_records_p, double threshold, uint8_t* __restrict__ low_score,                     \
+        float* __restrict__ probs, double* __restrict__ qual_out, double* __restrict__ phred_out, long long* counts,    \
+        unsigned chunk_nodes_cap, int phred_mode
+#define K3_INFER_ARGS \
+    plan, feats, row_stride, n_records_p, threshold, low_score, probs, qual_out, phred_out, counts, chunk_nodes_cap, phred_mode
+template <int TPB>
+__global__ void __launch_bounds__(TPB, 1) k3_infer(K3_INFER_PARAMS) {
+#ifdef UGVC_HOST_EMU
+    // the host emulation's launcher calls k3_infer for every plan: the walk is picked here (on the device, launch_k3 picks
+    // the kernel and this instantiation stays the plain one)
+    if (plan.walk == K3_WALK_CAT) {
+        k3_infer_run<TPB, K3_WALK_CAT>(K3_INFER_ARGS);
+        return;
+    }
+#endif
+    k3_infer_run<TPB, K3_WALK_PLAIN>(K3_INFER_ARGS);
+}
+template <int TPB>
+__global__ void __launch_bounds__(TPB, 1) k3_infer_cat(K3_INFER_PARAMS) { k3_infer_run<TPB, K3_WALK_CAT>(K3_INFER_ARGS); }
 
 #define K3_SMEM_BUDGET (224u * 1024u)
 
@@ -1305,16 +1372,47 @@ __device__ __forceinline__ void walkh(const uint8_t* __restrict__ s_node, const 
     for (int j = 0; j < NCH; ++j) leaf[j] = (int)s_leaf[(a8[j] >> 3) - H];
 }
 
+// walkh for K3_WALK_CAT plans: node = (threshold bits or UGVC_CAT_REF, byte offset of the feature | NODE_* flags << 30)
+template <int NCH>
+__device__ __forceinline__ void walkhc(const uint8_t* __restrict__ s_node, const uint16_t* __restrict__ s_leaf,
+                                       const uint32_t* __restrict__ s_cat, unsigned H, int depth, unsigned tr,
+                                       unsigned tr_end, const uint8_t* __restrict__ xcol, int leaf[NCH]) {
+    unsigned a8[NCH];
+    int go_l[NCH];
+#pragma unroll
+    for (int j = 0; j < NCH; ++j) {
+        const unsigned t = tr + j < tr_end ? tr + j : tr;  // pad with a repeat (result ignored)
+        const unsigned tb8 = t * H * 8u;
+        a8[j] = tb8 + 8u;
+        go_l[j] = -(int)tb8;
+    }
+    for (int d = 0; d < depth; ++d) {
+        uint2 nd[NCH];
+#pragma unroll
+        for (int j = 0; j < NCH; ++j) nd[j] = *reinterpret_cast<const uint2*>(s_node + a8[j]);
+#pragma unroll
+        for (int j = 0; j < NCH; ++j) {
+            const float xv = *reinterpret_cast<const float*>(xcol + (nd[j].y & 0x3FFFFFFFu));
+            const bool left = k3_cat_left(xv, nd[j].x, nd[j].y >> 30, s_cat);
+            const unsigned l8 = 2u * a8[j] + (unsigned)go_l[j];
+            a8[j] = left ? l8 : l8 + 8u;
+        }
+    }
+#pragma unroll
+    for (int j = 0; j < NCH; ++j) leaf[j] = (int)s_leaf[(a8[j] >> 3) - H];
+}
+
 // NBUF = 2: the raw rows of the NEXT record tile are fetched by 1-D bulk copies (cp.async.bulk, one per feature row,
 // completion on an mbarrier) while the current tile is walked, so no warp ever waits on HBM; every thread then turns
 // its own column of the landed slot words into feature values in place (K2's policies) -- a thread only ever reads
 // its own column, so the tile needs no barrier between assembly and walk.
-template <int TPB, int NBUF, int NCH, int GROUPS>
-__global__ void __launch_bounds__(TPB, 1)
-k3_heap(const __grid_constant__ DevPlan plan, const uint32_t* __restrict__ raw, const float* __restrict__ feats,
-        size_t row_stride, const int64_t* __restrict__ n_records_p, double threshold, uint8_t* __restrict__ low_score,
-        float* __restrict__ probs, double* __restrict__ qual_out, double* __restrict__ phred_out, long long* counts,
-        unsigned chunk_trees, int phred_mode, unsigned long long* err) {
+// k3_heap's body; WALK: K3_WALK_* (one kernel per walk, chosen by the launcher from plan.walk)
+template <int TPB, int NBUF, int NCH, int GROUPS, int WALK>
+__device__ __forceinline__ void
+k3_heap_run(const DevPlan& plan, const uint32_t* __restrict__ raw, const float* __restrict__ feats,
+            size_t row_stride, const int64_t* __restrict__ n_records_p, double threshold, uint8_t* __restrict__ low_score,
+            float* __restrict__ probs, double* __restrict__ qual_out, double* __restrict__ phred_out, long long* counts,
+            unsigned chunk_trees, int phred_mode, unsigned long long* err) {
     extern __shared__ __align__(16) uint8_t smem3[];
     const int F = plan.h.n_features, K = plan.h.n_classes, O = plan.h.n_outputs;
     const unsigned n_trees = plan.h.n_trees;
@@ -1329,12 +1427,20 @@ k3_heap(const __grid_constant__ DevPlan plan, const uint32_t* __restrict__ raw, 
     uint2* s_node = reinterpret_cast<uint2*>(reinterpret_cast<float*>(smem3) + (size_t)GROUPS * NBUF * F * GS);  // [chunk_trees][H]
     PlanFeature* s_pf = reinterpret_cast<PlanFeature*>(s_node + (forest ? (size_t)chunk_trees * H : 0));  // [F]
     uint16_t* s_leaf = reinterpret_cast<uint16_t*>(s_pf + F);                                              // [chunk_trees][H]
+    uint32_t* s_cat = reinterpret_cast<uint32_t*>(s_leaf + (size_t)chunk_trees * H);                        // [n_cat_words]
     const bool resident = forest && n_trees <= chunk_trees;  // whole forest fits: stage once
     for (int i = threadIdx.x; i < F; i += TPB) s_pf[i] = plan.feats[i];
+    if (WALK == K3_WALK_CAT) {
+        const uint32_t* cat = reinterpret_cast<const uint32_t*>(plan.dev_nodes + plan.h.n_nodes);
+        for (unsigned i = threadIdx.x; i < plan.n_cat_words; i += TPB) s_cat[i] = cat[i];
+    }
+    // K3_WALK_CAT: the node flags follow the features in heap_feat
+    const uint8_t* heap_flags = plan.heap_feat + (size_t)n_trees * H;
     if (resident) {
         const unsigned cnt = n_trees * H;
         for (unsigned i = threadIdx.x; i < cnt; i += TPB) {
-            s_node[i] = make_uint2(__float_as_uint(plan.heap_thr[i]), (unsigned)plan.heap_feat[i] * (unsigned)(GS * sizeof(float)));
+            const unsigned fl = WALK == K3_WALK_CAT ? (unsigned)heap_flags[i] << 30 : 0u;
+            s_node[i] = make_uint2(__float_as_uint(plan.heap_thr[i]), (unsigned)plan.heap_feat[i] * (unsigned)(GS * sizeof(float)) | fl);
             s_leaf[i] = plan.heap_leaf[i];
         }
     }
@@ -1452,8 +1558,9 @@ k3_heap(const __grid_constant__ DevPlan plan, const uint32_t* __restrict__ raw, 
                     const unsigned cnt = (c1 - c0) * H;
                     const size_t off = (size_t)c0 * H;
                     for (unsigned i = threadIdx.x; i < cnt; i += TPB) {
+                        const unsigned fl = WALK == K3_WALK_CAT ? (unsigned)heap_flags[off + i] << 30 : 0u;
                         s_node[i] = make_uint2(__float_as_uint(plan.heap_thr[off + i]),
-                                               (unsigned)plan.heap_feat[off + i] * (unsigned)(GS * sizeof(float)));
+                                               (unsigned)plan.heap_feat[off + i] * (unsigned)(GS * sizeof(float)) | fl);
                         s_leaf[i] = plan.heap_leaf[off + i];
                     }
                     __syncthreads();
@@ -1466,7 +1573,8 @@ k3_heap(const __grid_constant__ DevPlan plan, const uint32_t* __restrict__ raw, 
                     int leaf[NCH];
                     const unsigned lt = resident ? tr : tr - c0, lt_end = resident ? c1 : c1 - c0;
                     const uint8_t* xcol = reinterpret_cast<const uint8_t*>(x);
-                    if (plan.h.cmp_mode == CMP_LE) walkh<CMP_LE, NCH>(reinterpret_cast<const uint8_t*>(s_node), s_leaf, H, depth, lt, lt_end, xcol, leaf);
+                    if (WALK == K3_WALK_CAT) walkhc<NCH>(reinterpret_cast<const uint8_t*>(s_node), s_leaf, s_cat, H, depth, lt, lt_end, xcol, leaf);
+                    else if (plan.h.cmp_mode == CMP_LE) walkh<CMP_LE, NCH>(reinterpret_cast<const uint8_t*>(s_node), s_leaf, H, depth, lt, lt_end, xcol, leaf);
                     else walkh<CMP_LT, NCH>(reinterpret_cast<const uint8_t*>(s_node), s_leaf, H, depth, lt, lt_end, xcol, leaf);
                     if (plan.h.model_kind == MODEL_GB_SKLEARN && O == 1) {
                         // raw += learning_rate * leaf (pre-scaled on the host), fp64, tree order
@@ -1529,13 +1637,38 @@ k3_heap(const __grid_constant__ DevPlan plan, const uint32_t* __restrict__ raw, 
     }
 }
 
+#define K3_HEAP_PARAMS                                                                                                  \
+    const __grid_constant__ DevPlan plan, const uint32_t* __restrict__ raw, const float* __restrict__ feats,            \
+        size_t row_stride, const int64_t* __restrict__ n_records_p, double threshold, uint8_t* __restrict__ low_score,  \
+        float* __restrict__ probs, double* __restrict__ qual_out, double* __restrict__ phred_out, long long* counts,    \
+        unsigned chunk_trees, int phred_mode, unsigned long long* err
+#define K3_HEAP_ARGS \
+    plan, raw, feats, row_stride, n_records_p, threshold, low_score, probs, qual_out, phred_out, counts, chunk_trees, phred_mode, err
+template <int TPB, int NBUF, int NCH, int GROUPS>
+__global__ void __launch_bounds__(TPB, 1) k3_heap(K3_HEAP_PARAMS) {
+#ifdef UGVC_HOST_EMU
+    // as k3_infer: the host emulation's launcher calls k3_heap for every plan
+    if (plan.walk == K3_WALK_CAT) {
+        k3_heap_run<TPB, NBUF, NCH, GROUPS, K3_WALK_CAT>(K3_HEAP_ARGS);
+        return;
+    }
+#endif
+    k3_heap_run<TPB, NBUF, NCH, GROUPS, K3_WALK_PLAIN>(K3_HEAP_ARGS);
+}
+template <int TPB, int NBUF, int NCH, int GROUPS>
+__global__ void __launch_bounds__(TPB, 1) k3_heap_cat(K3_HEAP_PARAMS) {
+    k3_heap_run<TPB, NBUF, NCH, GROUPS, K3_WALK_CAT>(K3_HEAP_ARGS);
+}
+
 // shared-memory plan of k3_heap: records per CTA, tile buffers, trees per staged chunk
 static size_t k3h_tree_bytes(const DevPlan& plan) { return (size_t)(1u << plan.heap_depth) * 10u; }  // 8-byte nodes + leaf rows
 struct K3hShape {
     int tpb, nbuf, groups;
 };
-static size_t k3h_tile_bytes(const DevPlan& plan, K3hShape c) {  // all tile buffers of the CTA + the policy table
-    return (size_t)c.nbuf * plan.h.n_features * c.tpb * sizeof(float) + (size_t)plan.h.n_features * sizeof(PlanFeature) + 64;
+static size_t k3_cat_bytes(const DevPlan& plan) { return (size_t)plan.n_cat_words * sizeof(uint32_t); }  // resident
+static size_t k3h_tile_bytes(const DevPlan& plan, K3hShape c) {  // all tile buffers of the CTA + the policy table + bitsets
+    return (size_t)c.nbuf * plan.h.n_features * c.tpb * sizeof(float) + (size_t)plan.h.n_features * sizeof(PlanFeature) + 64 +
+           k3_cat_bytes(plan);
 }
 static K3hShape k3h_shape(const DevPlan& plan) {
     static const int force = getenv("UGVC_K3_SHAPE") ? atoi(getenv("UGVC_K3_SHAPE")) : -1;  // profiling knob: index below
@@ -1582,6 +1715,7 @@ K3Config k3_heap_config(const DevPlan& plan, int sm_count) {
     per_sm = per_sm < 1 ? 1 : (per_sm > 4 ? 4 : per_sm);
     if (per_sm * sh.tpb > 1536) per_sm = 1536 / sh.tpb;
     c.grid = sm_count * per_sm;
+    c.walk = (int)plan.walk;
     return c;
 }
 #ifndef UGVC_HOST_EMU
@@ -1590,9 +1724,16 @@ void launch_k3_fused(const DevPlan& plan, const uint32_t* raw, const float* feat
                      double* phreds, int phred_mode, long long* d_counts, unsigned long long* d_err, int sm_count,
                      cudaStream_t st) {
     const K3Config c = k3_heap_config(plan, sm_count);
-#define K3H_LAUNCH(T, B, C, G)                                                                                                  \
-    k3_heap<T, B, C, G><<<c.grid, T, c.smem, st>>>(plan, raw, feats, row_stride, d_n_records, threshold, low_score, probs, \
-                                                   qual, phreds, d_counts, c.chunk, phred_mode, d_err)
+#define K3H_LAUNCH(T, B, C, G)                                                                                             \
+    do {                                                                                                                   \
+        if (plan.walk == K3_WALK_CAT)                                                                                      \
+            k3_heap_cat<T, B, C, G><<<c.grid, T, c.smem, st>>>(plan, raw, feats, row_stride, d_n_records, threshold,        \
+                                                               low_score, probs, qual, phreds, d_counts, c.chunk,           \
+                                                               phred_mode, d_err);                                          \
+        else                                                                                                               \
+            k3_heap<T, B, C, G><<<c.grid, T, c.smem, st>>>(plan, raw, feats, row_stride, d_n_records, threshold, low_score, \
+                                                           probs, qual, phreds, d_counts, c.chunk, phred_mode, d_err);      \
+    } while (0)
     if (c.groups == 2 && c.tpb == 512) K3H_LAUNCH(512, 1, 8, 2);
     else if (c.groups == 2 && c.tpb == 448 && c.nch == 12) K3H_LAUNCH(448, 1, 12, 2);
     else if (c.groups == 2 && c.tpb == 448) K3H_LAUNCH(448, 1, 8, 2);
@@ -1614,7 +1755,7 @@ static size_t k3_roots_bytes(const DevPlan& plan) { return ((size_t)plan.h.n_tre
 static int k3_tpb(const DevPlan& plan) {
     const size_t forest = k3_forest_bytes(plan);
     if (forest == 0) return 256;
-    const size_t need384 = (size_t)plan.h.n_features * 384 * sizeof(float) + forest + k3_roots_bytes(plan);
+    const size_t need384 = (size_t)plan.h.n_features * 384 * sizeof(float) + forest + k3_roots_bytes(plan) + k3_cat_bytes(plan);
     static const int force = getenv("UGVC_K3_TPB") ? atoi(getenv("UGVC_K3_TPB")) : 0;  // profiling knob
     if (force == 256 || force == 384) return force == 384 && need384 > K3_SMEM_BUDGET ? 256 : force;
     return need384 <= K3_SMEM_BUDGET ? 384 : 256;
@@ -1623,7 +1764,7 @@ static int k3_tpb(const DevPlan& plan) {
 static unsigned k3_chunk_nodes(const DevPlan& plan) {
     if (k3_forest_bytes(plan) == 0) return 0;
     const size_t tile = (size_t)plan.h.n_features * k3_tpb(plan) * sizeof(float);
-    const size_t roots = k3_roots_bytes(plan);
+    const size_t roots = k3_roots_bytes(plan) + k3_cat_bytes(plan);  // the tree roots and the bitsets stay resident
     if (tile + roots + 4096 > K3_SMEM_BUDGET) return 0;
     const size_t room = (K3_SMEM_BUDGET - tile - roots) / sizeof(uint2);
     return (unsigned)(room < plan.h.n_nodes ? room : plan.h.n_nodes);
@@ -1631,7 +1772,7 @@ static unsigned k3_chunk_nodes(const DevPlan& plan) {
 size_t k3_smem_bytes(const DevPlan& plan) {
     size_t b = (size_t)plan.h.n_features * k3_tpb(plan) * sizeof(float);
     const unsigned cap = k3_chunk_nodes(plan);
-    if (cap) b += (size_t)cap * sizeof(uint2) + k3_roots_bytes(plan);
+    if (cap) b += (size_t)cap * sizeof(uint2) + k3_roots_bytes(plan) + k3_cat_bytes(plan);
     return b;
 }
 unsigned k3_chunk_nodes_cap(const DevPlan& plan) { return k3_chunk_nodes(plan); }
@@ -1639,9 +1780,10 @@ bool k3_plan_fits(const DevPlan& plan) {
     if (k3_forest_bytes(plan) == 0) return (size_t)plan.h.n_features * 256 * sizeof(float) <= K3_SMEM_BUDGET;
     return k3_chunk_nodes(plan) > 0;
 }
-// most features k3_infer holds for this model: a 256-record tile, plus for a forest the tree roots and 4 KiB of nodes
+// most features k3_infer holds for this model: a 256-record tile, plus for a forest the tree roots, the category
+// bitsets and 4 KiB of nodes
 unsigned k3_infer_max_features(const DevPlan& plan) {
-    const size_t fixed = k3_forest_bytes(plan) ? k3_roots_bytes(plan) + 4096 : 0;
+    const size_t fixed = k3_forest_bytes(plan) ? k3_roots_bytes(plan) + k3_cat_bytes(plan) + 4096 : 0;
     return fixed >= K3_SMEM_BUDGET ? 0u : (unsigned)((K3_SMEM_BUDGET - fixed) / (256 * sizeof(float)));
 }
 K3Config k3_infer_config(const DevPlan& plan, int sm_count) {
@@ -1657,6 +1799,7 @@ K3Config k3_infer_config(const DevPlan& plan, int sm_count) {
     if (per_sm < 1) per_sm = 1;
     if (per_sm > 4) per_sm = 4;
     c.grid = sm_count * per_sm;
+    c.walk = (int)plan.walk;
     return c;
 }
 
@@ -1665,12 +1808,14 @@ void launch_k3(const DevPlan& plan, const float* feats, size_t row_stride, const
                double threshold, uint8_t* low_score, float* probs, double* qual, double* phreds, int phred_mode,
                long long* d_counts, int sm_count, cudaStream_t st) {
     const K3Config c = k3_infer_config(plan, sm_count);
-    if (c.tpb == 384)
-        k3_infer<384><<<c.grid, 384, c.smem, st>>>(plan, feats, row_stride, d_n_records, threshold, low_score,
-                                                   probs, qual, phreds, d_counts, c.chunk, phred_mode);
-    else
-        k3_infer<256><<<c.grid, 256, c.smem, st>>>(plan, feats, row_stride, d_n_records, threshold, low_score,
-                                                   probs, qual, phreds, d_counts, c.chunk, phred_mode);
+#define K3I_LAUNCH(K, T) \
+    K<T><<<c.grid, T, c.smem, st>>>(plan, feats, row_stride, d_n_records, threshold, low_score, probs, qual, phreds, d_counts, \
+                                   c.chunk, phred_mode)
+    if (plan.walk == K3_WALK_CAT && c.tpb == 384) K3I_LAUNCH(k3_infer_cat, 384);
+    else if (plan.walk == K3_WALK_CAT) K3I_LAUNCH(k3_infer_cat, 256);
+    else if (c.tpb == 384) K3I_LAUNCH(k3_infer, 384);
+    else K3I_LAUNCH(k3_infer, 256);
+#undef K3I_LAUNCH
 }
 
 cudaError_t kernels_configure(const DevPlan& plan) {
@@ -1698,8 +1843,21 @@ cudaError_t kernels_configure(const DevPlan& plan) {
         if ((e = cudaFuncSetAttribute(k3_heap<256, 1, 8, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim)) != cudaSuccess) return e;
         if ((e = cudaFuncSetAttribute(k3_heap<128, 2, 16, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim)) != cudaSuccess) return e;
         if ((e = cudaFuncSetAttribute(k3_heap<128, 1, 8, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim)) != cudaSuccess) return e;
+        if ((e = cudaFuncSetAttribute(k3_heap_cat<512, 1, 8, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim)) != cudaSuccess) return e;
+        if ((e = cudaFuncSetAttribute(k3_heap_cat<384, 1, 16, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim)) != cudaSuccess) return e;
+        if ((e = cudaFuncSetAttribute(k3_heap_cat<448, 1, 8, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim)) != cudaSuccess) return e;
+        if ((e = cudaFuncSetAttribute(k3_heap_cat<448, 1, 12, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim)) != cudaSuccess) return e;
+        if ((e = cudaFuncSetAttribute(k3_heap_cat<256, 2, 16, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim)) != cudaSuccess) return e;
+        if ((e = cudaFuncSetAttribute(k3_heap_cat<192, 2, 16, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim)) != cudaSuccess) return e;
+        if ((e = cudaFuncSetAttribute(k3_heap_cat<256, 1, 8, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim)) != cudaSuccess) return e;
+        if ((e = cudaFuncSetAttribute(k3_heap_cat<128, 2, 16, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim)) != cudaSuccess) return e;
+        if ((e = cudaFuncSetAttribute(k3_heap_cat<128, 1, 8, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim)) != cudaSuccess) return e;
     }
     e = cudaFuncSetAttribute(k3_infer<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
+    if (e != cudaSuccess) return e;
+    e = cudaFuncSetAttribute(k3_infer_cat<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
+    if (e != cudaSuccess) return e;
+    e = cudaFuncSetAttribute(k3_infer_cat<384>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
     if (e != cudaSuccess) return e;
     return cudaFuncSetAttribute(k3_infer<384>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
 }

@@ -21,8 +21,11 @@ struct DevPlan {
     const uint32_t* tree_root;
     const uint8_t* tree_out;
     const PlanNode* nodes;     // blob form (host validation)
-    const uint2* dev_nodes;    // device form: x = threshold bits (leaf: quiet NaN | leaf row), y = feature | right_abs << 8
+    const uint2* dev_nodes;    // device form: x = threshold bits (leaf: quiet NaN | leaf row; categorical node: UGVC_CAT_REF),
+                               // y = feature | right_abs << 8 (K3_WALK_CAT: feature | NODE_* flags << 8 | right_abs << 10);
+                               // the n_cat_words category bitset words follow the n_nodes nodes
     uint32_t max_depth;        // deepest leaf over all trees
+    uint32_t walk;             // K3_WALK_*: which tree walk K3 runs (in what was padding: the layout is unchanged)
     const double* leaves;
     // heap form of the forest (k3_heap): every tree padded to a complete binary tree of depth heap_depth,
     // node i at index i (root 1, children 2i / 2i+1), H = 2^heap_depth entries per tree and array
@@ -30,9 +33,13 @@ struct DevPlan {
     const uint8_t* heap_feat;  // [n_trees][H] feature of the node
     const uint16_t* heap_leaf; // [n_trees][H] leaf row reached from node 2^depth + k
     uint32_t heap_depth;       // 0: the forest has no heap form (too deep / too many leaf rows): k2 + k3_infer
+    uint32_t n_cat_words;      // category bitset words (after dev_nodes); K3 stages them all in shared memory
     const uint8_t* htab;       // 256-entry open-addressing table: tag index or 0xFF
     uint32_t first_fixed_slot; // slots [first_fixed_slot, n_slots) are TAG_FIXED
 };
+// K3's tree walks.  PLAIN: a row goes left when x < / <= threshold (NaN goes right).  CAT (xgboost plans with
+// default-left or categorical nodes, plan.h NODE_*): NaN to the default child, categorical sets from the bitsets.
+enum : uint32_t { K3_WALK_PLAIN = 0, K3_WALK_CAT = 1 };
 
 // Learned key order ("schedule"): the INFO keys in the order records carry them and the usual
 // FORMAT column.  K1 steps through it warp-uniformly, matching "KEY=" word-wise against the
@@ -195,6 +202,7 @@ struct K3Config {
     bool resident;          // the whole model is staged once (no chunk loop)
     size_t smem;            // dynamic shared memory per CTA
     int grid;               // CTAs of the persistent grid
+    int walk;               // K3_WALK_* of the instantiation that runs
 };
 K3Config k3_heap_config(const DevPlan& plan, int sm_count);   // only when k3_fused_available(plan)
 K3Config k3_infer_config(const DevPlan& plan, int sm_count);

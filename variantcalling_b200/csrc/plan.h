@@ -8,7 +8,7 @@
 #include <stdint.h>
 
 #define UGVC_PLAN_MAGIC 0x50564755u /* "UGVP" */
-#define UGVC_PLAN_VERSION 8u
+#define UGVC_PLAN_VERSION 9u
 
 #define UGVC_MAX_TAGS 128
 #define UGVC_MAX_SLOTS 250
@@ -149,13 +149,37 @@ struct alignas(4) PlanCombine {  // 8 bytes: feature = max(feature, slot_b) skip
 };
 
 struct alignas(8) PlanNode {  // 8 bytes, preorder layout: left child = this + 1
-    float value;              // internal: threshold (fp32); leaf: bit pattern of the int32 leaf row
+    float value;              // internal: threshold (fp32); categorical: bit pattern of UGVC_CAT_REF(first word, words);
+                              // leaf: bit pattern of the int32 leaf row
     int16_t feature;          // < 0 for a leaf
     uint16_t right;           // index of the right child relative to the tree root
 };
+
+// ---- per-node flags of a forest (xgboost only; zero for sklearn models and on leaves) -------------
+// xgboost 2.1.2's CPU predictor (GetNextNode / common::Decision), restated, PARITY UNPINNED (xgboost is not
+// installed where this is built):
+//   NaN goes to the default child (left when NODE_DEFAULT_LEFT is set, else right), at every node kind;
+//   numeric node: left when fp32 x < threshold;
+//   categorical node: left when x < 0 or x >= 2^24 (invalid category), or when int(x) (truncated) is not in the
+//   node's category set; right when it is.  The set is a bitset: bit c of word c / 32 of the node's words.
+enum : uint8_t {
+    NODE_DEFAULT_LEFT = 1,
+    NODE_CATEGORICAL = 2,
+};
+// Categories are codes in [0, UGVC_MAX_CATEGORIES): a node's bitset has at most UGVC_MAX_CATEGORIES / 32 words.
+#define UGVC_MAX_CATEGORIES 1024u
+#define UGVC_CAT_MAX_WORDS (UGVC_MAX_CATEGORIES / 32u)
+#define UGVC_CAT_REF(first, words) ((uint32_t)(first) | ((uint32_t)(words) << 24))  // first word < 2^24
+#define UGVC_CAT_FIRST(ref) ((ref) & 0xFFFFFFu)
+#define UGVC_CAT_WORDS(ref) ((ref) >> 24)
+
+struct alignas(8) PlanCatHeader {  // 8 bytes: opens the category section of a forest
+    uint32_t n_words;              // uint32 bitset words that follow
+    uint32_t n_flagged;            // nodes with a non-zero flag byte (0: the plain walk runs)
+};
 static_assert(sizeof(PlanHeader) == 96 && sizeof(PlanTag) == 40 && sizeof(PlanSlot) == 4 && sizeof(PlanDict) == 4 &&
                   sizeof(PlanString) == 32 && sizeof(PlanFeature) == 12 && sizeof(PlanCheck) == 8 &&
-                  sizeof(PlanCombine) == 8 && sizeof(PlanNode) == 8,
+                  sizeof(PlanCombine) == 8 && sizeof(PlanNode) == 8 && sizeof(PlanCatHeader) == 8,
               "plan record layout");
 
 // Hash of a tag name held as four little-endian 64-bit words (+ length); the host builds the
@@ -177,4 +201,6 @@ static inline unsigned ugvc_key_hash(unsigned long long k0, unsigned long long k
 //   PlanFeature[n_features], PlanCheck[n_checks], PlanCombine[n_combines],
 //   MODEL_LOGISTIC : double coef[n_outputs * n_features], double intercept[n_outputs]
 //   forests        : uint32 tree_root[n_trees + 1], uint8 tree_out[n_trees] (output column of each tree),
-//                    PlanNode[n_nodes], double leaves[n_leaf_rows * leaf_width]
+//                    PlanNode[n_nodes], double leaves[n_leaf_rows * leaf_width],
+//                    uint8 node_flags[n_nodes] (NODE_*), PlanCatHeader, uint32 cat_words[n_words]
+//                    (a categorical node's PlanNode.value holds UGVC_CAT_REF of its words in cat_words)

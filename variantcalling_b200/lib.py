@@ -423,11 +423,11 @@ class Context:
 
     def k3_config(self) -> dict:
         """The K3 launch the loaded plan gets (test hook ugvc_test_k3_config)."""
-        out = np.zeros(8, np.int32)
+        out = np.zeros(9, np.int32)
         self._check(self.lib.ugvc_test_k3_config(self.h, _ptr(out)))
-        kernel, tpb, nbuf, groups, nch, chunk, resident, grid = (int(v) for v in out)
+        kernel, tpb, nbuf, groups, nch, chunk, resident, grid, walk = (int(v) for v in out)
         return {"kernel": ("heap", "infer")[kernel], "tpb": tpb, "nbuf": nbuf, "groups": groups, "nch": nch, "chunk": chunk,
-                "resident": bool(resident), "grid": grid, "gs": tpb // groups}
+                "resident": bool(resident), "grid": grid, "gs": tpb // groups, "walk": ("plain", "categorical")[walk]}
 
     def enable_stage_timing(self, on: bool = True):
         self._check(self.lib.ugvc_enable_stage_timing(self.h, int(on)))

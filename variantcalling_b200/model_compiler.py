@@ -35,7 +35,7 @@ import numpy as np
 from variantcalling_b200.vcf_header import VcfHeader
 
 PLAN_MAGIC = 0x50564755
-PLAN_VERSION = 8
+PLAN_VERSION = 9
 MAX_TAGS, MAX_SLOTS, MAX_FEATURES, MAX_CLASSES, NAME_MAX = 128, 250, 250, 4, 32
 MAX_DICTS, MAX_STRINGS = 64, 96
 
@@ -47,6 +47,8 @@ TAG_FIXED, ELEM_WHOLE = 0xFF, 0xFF
 POL_VALUE, POL_ERROR, POL_NULL = 0, 1, 2
 MODEL_LOGISTIC, MODEL_GB_SKLEARN, MODEL_RF_SKLEARN, MODEL_XGB = 1, 2, 3, 4
 CMP_LE, CMP_LT = 0, 1
+NODE_DEFAULT_LEFT, NODE_CATEGORICAL = 1, 2
+MAX_CATEGORIES = 1024  # category codes in [0, 1024): a node's bitset has at most 32 words (plan.h UGVC_MAX_CATEGORIES)
 
 
 class PlanError(ValueError):
@@ -344,8 +346,9 @@ def _f32_floor(t: np.ndarray) -> np.ndarray:
     return f
 
 
-def _preorder_tree(left, right, feature, thr32, leaf_row_of):
-    """Child arrays (-1 = leaf) -> preorder node list [(is_leaf, thr | leaf_row, feature, right_rel)]."""
+def _preorder_tree(left, right, feature, thr32, leaf_row_of, node_kind=None):
+    """Child arrays (-1 = leaf) -> preorder node list [(is_leaf, thr | leaf_row, feature, right_rel, flags, cat_ref)].
+    ``node_kind(n)`` -> (NODE_* flags, category bitset reference or None) of an internal node (default: (0, None))."""
     order, seq, stack = {}, [], [0]
     while stack:  # iterative DFS, left subtree first => left child is always the next node
         n = stack.pop()
@@ -359,29 +362,90 @@ def _preorder_tree(left, right, feature, thr32, leaf_row_of):
     nodes = []
     for n in seq:
         if left[n] == -1:
-            nodes.append((True, int(leaf_row_of(n)), -1, 0))
+            nodes.append((True, int(leaf_row_of(n)), -1, 0, 0, None))
         else:
             if order[int(left[n])] != order[n] + 1:
                 raise PlanError("internal error: preorder layout violated")
-            nodes.append((False, float(thr32[n]), int(feature[n]), order[int(right[n])]))
+            flags, cat_ref = node_kind(n) if node_kind is not None else (0, None)
+            nodes.append((False, float(thr32[n]), int(feature[n]), order[int(right[n])], flags, cat_ref))
     return nodes
 
 
-def _pack_forest(trees, tree_out, leaves, leaf_width) -> tuple[bytes, int, int]:
+def _pack_forest(trees, tree_out, leaves, leaf_width, cat_words=()) -> tuple[bytes, int, int]:
+    """Forest section (plan.h): roots, tree outputs, preorder nodes, leaves, node flags, category bitset words."""
     roots = [0]
     node_bytes = bytearray()
+    flags = bytearray()
     for nodes in trees:
-        for is_leaf, value, feat, right in nodes:
+        for is_leaf, value, feat, right, fl, cat_ref in nodes:
             if is_leaf:
                 node_bytes += struct.pack("<ihH", value, -1, 0)
+            elif cat_ref is not None:
+                node_bytes += struct.pack("<IhH", cat_ref, feat, right)
             else:
                 node_bytes += struct.pack("<fhH", value, feat, right)
+            flags.append(fl)
         roots.append(roots[-1] + len(nodes))
     out = _pad8(np.asarray(roots, dtype="<u4").tobytes())
     out += _pad8(np.asarray(tree_out, dtype=np.uint8).tobytes())
     out += _pad8(bytes(node_bytes))
     out += _pad8(np.asarray(leaves, dtype="<f8").tobytes())
+    out += _pad8(bytes(flags))
+    out += struct.pack("<II", len(cat_words), sum(1 for f in flags if f))
+    out += _pad8(np.asarray(cat_words, dtype="<u4").tobytes())
     return out, roots[-1], len(leaves) // max(1, leaf_width)
+
+
+def _xgb_node_kinds(tr, ti: int, cat_words: list, bitset_at: dict):
+    """-> node_kind(n) for _preorder_tree: the default-left / categorical flags of one xgboost tree, its category sets
+    appended to ``cat_words`` as bitsets (bit c of word c // 32), each distinct bitset once (``bitset_at``: words ->
+    first word).  A malformed category section raises PlanError."""
+    n_nodes = len(tr["left_children"])
+    split_type = np.asarray(tr.get("split_type") or [0] * n_nodes, dtype=np.int64)
+    default_left = np.asarray(tr.get("default_left") or [0] * n_nodes, dtype=np.int64)
+    if split_type.size != n_nodes or default_left.size != n_nodes:
+        raise PlanError(f"xgboost tree {ti}: split_type / default_left do not have one entry per node")
+    if ((split_type != 0) & (split_type != 1)).any():
+        raise PlanError(f"xgboost tree {ti}: unknown split_type (0 numeric, 1 categorical)")
+    cats = [int(c) for c in tr.get("categories", [])]
+    c_nodes = [int(c) for c in tr.get("categories_nodes", [])]
+    c_seg = [int(c) for c in tr.get("categories_segments", [])]
+    c_size = [int(c) for c in tr.get("categories_sizes", [])]
+    if not len(c_nodes) == len(c_seg) == len(c_size):
+        raise PlanError(f"xgboost tree {ti}: categories_nodes / _segments / _sizes differ in length")
+    ref_of = {}
+    for nid, seg, size in zip(c_nodes, c_seg, c_size):
+        if not 0 <= nid < n_nodes or split_type[nid] != 1:
+            raise PlanError(f"xgboost tree {ti}: categories_nodes names node {nid}, which is not a categorical split")
+        if seg < 0 or size < 1 or seg + size > len(cats):
+            raise PlanError(f"xgboost tree {ti}: category segment [{seg}, {seg}+{size}) of node {nid} is out of range "
+                            f"({len(cats)} categories)")
+        codes = cats[seg:seg + size]
+        if min(codes) < 0:
+            raise PlanError(f"xgboost tree {ti}: node {nid} has a negative category code")
+        if max(codes) >= MAX_CATEGORIES:
+            raise PlanError(f"xgboost tree {ti}: node {nid} has category code {max(codes)}; codes must be below "
+                            f"{MAX_CATEGORIES} (the category limit of the plan)")
+        words = [0] * (max(codes) // 32 + 1)
+        for c in codes:
+            words[c // 32] |= 1 << (c % 32)
+        key = tuple(words)
+        if key not in bitset_at:
+            if len(cat_words) + len(words) >= 1 << 24:
+                raise PlanError("too many category bitset words")
+            bitset_at[key] = len(cat_words)
+            cat_words.extend(words)
+        ref_of[nid] = bitset_at[key] | (len(words) << 24)
+    left = tr["left_children"]
+    for nid in range(n_nodes):
+        if split_type[nid] == 1 and left[nid] != -1 and nid not in ref_of:
+            raise PlanError(f"xgboost tree {ti}: categorical node {nid} is missing from categories_nodes")
+
+    def node_kind(n):
+        fl = (NODE_DEFAULT_LEFT if default_left[n] else 0) | (NODE_CATEGORICAL if split_type[n] == 1 else 0)
+        return fl, ref_of.get(n)
+
+    return node_kind
 
 
 def _lower_model(model, n_features: int) -> dict:  # noqa: C901, PLR0912, PLR0915
@@ -475,8 +539,13 @@ def _lower_model(model, n_features: int) -> dict:  # noqa: C901, PLR0912, PLR091
 def _lower_xgboost_json(doc, n_features: int) -> dict:
     """xgboost >= 1.x ``Booster.save_model('*.json')`` document (gbtree, binary:logistic or
     multi:softprob).  PARITY UNPINNED: xgboost is not installed in the build container; the
-    algorithm restated is xgboost's published CPU predictor (fp32 ``x < split_condition`` goes
-    left, fp32 margin accumulated in tree order from logit(base_score), fp32 sigmoid/softmax)."""
+    algorithm restated is xgboost 2.1.2's CPU predictor (fp32 ``x < split_condition`` goes
+    left, fp32 margin accumulated in tree order from logit(base_score), fp32 sigmoid/softmax),
+    with its missing-value and categorical routing (``GetNextNode`` / ``common::Decision``): NaN
+    takes the node's default child (``default_left``); a categorical node (``split_type`` 1, its set
+    in ``categories[categories_segments[i]:][:categories_sizes[i]]``) sends a category in the set
+    right and everything else (not in the set, negative, >= 2^24) left.  Category codes must be
+    below ``MAX_CATEGORIES``."""
     if isinstance(doc, (str, bytes)):
         try:
             doc = json.loads(doc)
@@ -508,8 +577,9 @@ def _lower_xgboost_json(doc, n_features: int) -> dict:
             init[o] = float(base_score)
     else:
         raise PlanError(f"xgboost objective {objective} is not lowered")
-    trees, tree_out, leaves = [], [], []
+    trees, tree_out, leaves, cat_words, bitset_at = [], [], [], [], {}
     for ti, tr in enumerate(model["trees"]):
+        node_kind = _xgb_node_kinds(tr, ti, cat_words, bitset_at)
         left = np.asarray(tr["left_children"], dtype=np.int64)
         right = np.asarray(tr["right_children"], dtype=np.int64)
         feat = np.asarray(tr["split_indices"], dtype=np.int64)
@@ -525,9 +595,9 @@ def _lower_xgboost_json(doc, n_features: int) -> dict:
                 leaves.append(float(cond[n]))
             return leaf_ids[n]
 
-        trees.append(_preorder_tree(left, right, feat, cond, leaf_row))
+        trees.append(_preorder_tree(left, right, feat, cond, leaf_row, node_kind))
         tree_out.append(int(tree_info[ti]) if n_out > 1 else 0)
-    section, n_nodes, n_rows = _pack_forest(trees, tree_out, leaves, 1)
+    section, n_nodes, n_rows = _pack_forest(trees, tree_out, leaves, 1, cat_words)
     return dict(kind=MODEL_XGB, n_classes=k, n_outputs=n_out, init=init, cmp=CMP_LT, section=section,
                 n_trees=len(trees), n_nodes=n_nodes, n_leaf_rows=n_rows, leaf_width=1, classes=list(range(k)))
 
