@@ -1,8 +1,9 @@
 // tests/host_emu/emu_kernels.cpp -- TEST INFRASTRUCTURE.  The K1 (field parse), K2 (feature assembly)
 // and K3 (inference) kernel bodies of variantcalling_b200/csrc/kernels.cu, compiled unchanged for the
 // host through shim_include/cuda_runtime.h with one emulated thread per CTA, plus host launchers
-// with the product's launch_* signatures.  K0 (a cooperative 256-thread tile scan with inline PTX)
-// is not emulated: lines are indexed by a plain loop that reproduces its outputs and error codes.
+// with the product's launch_* signatures (K3's is in kernels.cu, next to the device launcher).
+// K0 (a cooperative 256-thread tile scan with inline PTX) is not emulated: lines are indexed by a
+// plain loop that reproduces its outputs and error codes.
 // The emulated library lets `pytest -m "not gpu"` run the parity tests against the very kernel
 // source the GPU executes; it is built under tests/ only and the package never loads it.
 #define UGVC_HOST_EMU 1
@@ -90,38 +91,6 @@ void launch_k2(const DevPlan& plan, const uint32_t* raw, size_t row_stride, cons
                unsigned long long* d_err, int, cudaStream_t) {
     one_thread_grid();
     k2_features(plan, raw, row_stride, d_n_records, feats, d_err);
-}
-
-void launch_k3(const DevPlan& plan, const float* feats, size_t row_stride, const int64_t* d_n_records, double threshold,
-               uint8_t* low_score, float* probs, double* qual, double* phreds, int phred_mode, long long* d_counts, int,
-               cudaStream_t) {
-    one_thread_grid();
-    // the product's forest buffer: a forest larger than it runs the chunk loop here too
-    const unsigned chunk = k3_infer_config(plan, 1).chunk;
-    const size_t need = (size_t)plan.h.n_features * sizeof(float) + (size_t)chunk * sizeof(uint2) +
-                        ((size_t)plan.h.n_trees + 2) * sizeof(uint32_t);
-    if (need > sizeof(smem3)) {
-        fprintf(stderr, "host_emu: forest too large for the emulated shared memory\n");
-        abort();
-    }
-    k3_infer<1>(plan, feats, row_stride, d_n_records, threshold, low_score, probs, qual, phreds, d_counts, chunk,
-                phred_mode);
-}
-
-void launch_k3_fused(const DevPlan& plan, const uint32_t* raw, const float* feats, size_t row_stride,
-                     const int64_t* d_n_records, double threshold, uint8_t* low_score, float* probs, double* qual,
-                     double* phreds, int phred_mode, long long* d_counts, unsigned long long* d_err, int, cudaStream_t) {
-    one_thread_grid();
-    // trees per staged chunk as the product's shape gives them: a forest larger than it runs the chunk loop here too
-    const unsigned chunk = k3_heap_config(plan, 1).chunk;
-    const size_t need = (size_t)plan.h.n_features * (sizeof(float) + sizeof(PlanFeature)) + 64 +
-                        (size_t)chunk * ((size_t)10 << plan.heap_depth) + 64;
-    if (need > sizeof(smem3)) {
-        fprintf(stderr, "host_emu: forest too large for the emulated shared memory\n");
-        abort();
-    }
-    k3_heap<1, 1, 8, 1>(plan, raw, feats, row_stride, d_n_records, threshold, low_score, probs, qual, phreds, d_counts,
-                        chunk, phred_mode, d_err);
 }
 
 cudaError_t kernels_configure(const DevPlan&) { return cudaSuccess; }

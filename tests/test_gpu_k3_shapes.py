@@ -1,6 +1,6 @@
 """GPU: K3 in every launch configuration it has, against the estimators themselves.
 
-The K3 launch depends on the model (kernels.cu: k3_fused_available, k3h_shape, k3h_chunk_trees, k3_tpb,
+The K3 launch depends on the model (kernels.cu: k3_choose, k3h_shape, k3h_chunk_trees, k3_tpb,
 k3_chunk_nodes): k3_heap in one of nine template shapes with the forest resident or staged in chunks of trees,
 or k3_infer (forests deeper than 8 or with >= 65536 leaf rows) with the forest resident or staged in chunks of
 nodes.  Every case below is sized to land on one configuration and asserts it through ugvc_test_k3_config, then

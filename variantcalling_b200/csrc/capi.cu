@@ -67,6 +67,7 @@ struct ugvc_ctx {
     std::string err;
     bool has_plan = false;
     DevPlan plan{};
+    K3Config k3{};                 // the K3 launch of the plan's model (k3_choose at load)
     uint8_t* d_plan = nullptr;
     uint8_t* d_htab = nullptr;
     uint2* d_nodes = nullptr;
@@ -111,15 +112,6 @@ static int fail(ugvc_ctx* ctx, int code, const std::string& msg) {
         if (_e != cudaSuccess)                                                                     \
             return fail(ctx, UGVC_E_CUDA, std::string(#call) + ": " + cudaGetErrorString(_e));     \
     } while (0)
-
-// UGVC_K3_LEGACY=1 (profiling): K2 + k3_infer even where k3_heap would run
-static bool k3_legacy() {
-    static const bool legacy = getenv("UGVC_K3_LEGACY") && *getenv("UGVC_K3_LEGACY") != '0';
-    return legacy;
-}
-// the K3 kernel of a plan with a model: k3_heap (K2 fused into its tile load) when the model has a heap form,
-// else K2 + k3_infer
-static bool k3_runs_heap(const DevPlan& p) { return !k3_legacy() && k3_fused_available(p); }
 
 extern "C" int ugvc_version(void) { return UGVC_VERSION; }
 
@@ -669,22 +661,10 @@ extern "C" int ugvc_load_plan(ugvc_ctx* ctx, const void* blob, size_t n_bytes) {
     p.first_fixed_slot = first_fixed;
     if (k1_smem_bytes(p) > 227 * 1024)
         return fail(ctx, UGVC_E_PLAN, "plan needs more shared memory than one sm_90 CTA has (K1 field parse)");
-    // the shared-memory limits are those of the K3 kernel that will run the model: k3_heap holds every plan the
-    // compiler makes (up to 250 features) when the model has a heap form, k3_infer fewer features
-    if (h.model_kind != MODEL_NONE && !k3_runs_heap(p)) {
-        if (k3_smem_bytes(p) > 227 * 1024 || !k3_plan_fits(p))
-            return fail(ctx, UGVC_E_PLAN,
-                        std::string("plan needs more shared memory than one sm_90 CTA has: k3_infer (") +
-                            (k3_legacy() ? "selected by UGVC_K3_LEGACY" : "forests deeper than 8 or with 65536 leaf rows or more") +
-                            ") holds at most " + std::to_string(k3_infer_max_features(p)) + " features for this model, it has " +
-                            std::to_string(h.n_features));
-        if (h.model_kind != MODEL_LOGISTIC) {
-            const uint32_t* root = reinterpret_cast<const uint32_t*>(hb + o_root);
-            const unsigned cap = k3_chunk_nodes_cap(p);
-            for (uint32_t t = 0; t < h.n_trees; ++t)
-                if (root[t + 1] - root[t] > cap)
-                    return fail(ctx, UGVC_E_PLAN, "a single tree does not fit k3_infer's shared-memory forest buffer");
-        }
+    if (h.model_kind != MODEL_NONE) {
+        std::string why;
+        if (!k3_choose(p, reinterpret_cast<const uint32_t*>(hb + o_root), ctx->sm_count, &ctx->k3, &why))
+            return fail(ctx, UGVC_E_PLAN, why);
     }
     CU(kernels_configure(p));
     ctx->h_tags.assign(tags, tags + h.n_tags);
@@ -915,16 +895,12 @@ static int enqueue_kernels(ugvc_ctx* ctx, Lane& l, const uint8_t* d_text, size_t
                   ctx->d_counts, ctx->sm_count, st);
     if (timing) CU(cudaEventRecord(ev[2], st));
     const bool has_model = p.h.model_kind != MODEL_NONE;
-    const bool fused = has_model && k3_runs_heap(p);
+    const bool fused = has_model && ctx->k3.kernel == K3_KERNEL_HEAP;  // features assembled in k3_heap's tile load
     if (has_model && !fused) launch_k2(p, l.b.raw, l.b.cap_records, d_n_records, l.b.feats, l.d_err, ctx->sm_count, st);
     if (timing) CU(cudaEventRecord(ev[3], st));
-    if (fused)  // feature assembly happens in the tile load of the inference kernel
-        launch_k3_fused(p, l.b.raw, nullptr, l.b.cap_records, d_n_records, threshold, d_low, d_probs, d_qual,
-                        d_low == l.b.low_score ? l.b.phreds : nullptr, ctx->want_phreds, ctx->d_counts, l.d_err,
-                        ctx->sm_count, st);
-    else if (has_model)
-        launch_k3(p, l.b.feats, l.b.cap_records, d_n_records, threshold, d_low, d_probs, d_qual,
-                  d_low == l.b.low_score ? l.b.phreds : nullptr, ctx->want_phreds, ctx->d_counts, ctx->sm_count, st);
+    if (has_model)
+        launch_k3(p, ctx->k3, l.b.raw, l.b.feats, l.b.cap_records, d_n_records, threshold, d_low, d_probs, d_qual,
+                  d_low == l.b.low_score ? l.b.phreds : nullptr, ctx->want_phreds, ctx->d_counts, l.d_err, st);
     if (timing) CU(cudaEventRecord(ev[4], st));
     ctx->launches += (has_model ? (fused ? 1 : 2) : 0) + (fast ? 2 : 2 + (p.h.n_slots ? 1 : 0));
     CU(cudaGetLastError());
@@ -1461,12 +1437,8 @@ extern "C" int ugvc_predict_features(ugvc_ctx* ctx, const float* x, size_t n, si
                          cudaMemcpyHostToDevice, st));
     const int64_t n64 = (int64_t)n;
     CU(cudaMemcpyAsync(l.b.n_records, &n64, sizeof(n64), cudaMemcpyHostToDevice, st));
-    if (k3_runs_heap(p))
-        launch_k3_fused(p, nullptr, l.b.feats, l.b.cap_records, l.b.n_records, threshold, l.b.low_score, l.b.probs, l.b.qual,
-                        l.b.phreds, ctx->want_phreds, ctx->d_counts, l.d_err, ctx->sm_count, st);
-    else
-        launch_k3(p, l.b.feats, l.b.cap_records, l.b.n_records, threshold, l.b.low_score, l.b.probs, l.b.qual,
-                  l.b.phreds, ctx->want_phreds, ctx->d_counts, ctx->sm_count, st);
+    launch_k3(p, ctx->k3, nullptr, l.b.feats, l.b.cap_records, l.b.n_records, threshold, l.b.low_score, l.b.probs, l.b.qual,
+              l.b.phreds, ctx->want_phreds, ctx->d_counts, l.d_err, st);
     ctx->launches += 1;
     CU(cudaGetLastError());
     if (out_low_score) CU(cudaMemcpyAsync(out_low_score, l.b.low_score, n, cudaMemcpyDeviceToHost, st));
@@ -1597,12 +1569,11 @@ extern "C" int ugvc_test_device_sigmoid(ugvc_ctx*, const float*, int, float*, fl
 #endif
 
 extern "C" int ugvc_test_k3_config(ugvc_ctx* ctx, int32_t out[9]) {
-    // test hook: the K3 launch the loaded plan gets, from the functions the launchers use
+    // test hook: the K3 launch the loaded plan gets
     if (!ctx || !out) return UGVC_E_ARG;
     if (!ctx->has_plan || ctx->plan.h.model_kind == MODEL_NONE)
         return fail(ctx, UGVC_E_STATE, "test_k3_config: load a plan with a model first");
-    const DevPlan& p = ctx->plan;
-    const K3Config c = k3_runs_heap(p) ? k3_heap_config(p, ctx->sm_count) : k3_infer_config(p, ctx->sm_count);
+    const K3Config& c = ctx->k3;
     const int32_t v[9] = {c.kernel, c.tpb, c.nbuf, c.groups, c.nch, (int32_t)c.chunk, c.resident ? 1 : 0, c.grid, c.walk};
     memcpy(out, v, sizeof(v));
     return UGVC_OK;

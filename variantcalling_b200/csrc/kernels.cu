@@ -23,6 +23,10 @@
 #include <math.h>
 #include <stdlib.h>
 
+#include <array>
+#include <iterator>
+#include <utility>
+
 #include "numparse.h"
 
 // UGVC_HOST_EMU: tests/host_emu compiles the K1-K3 kernel bodies of this file with g++ (one emulated
@@ -1177,13 +1181,13 @@ __device__ __forceinline__ bool k3_finish(const DevPlan& plan, const float* __re
     return low;
 }
 
-// k3_infer's body; WALK: K3_WALK_* (one kernel per walk, chosen by the launcher from plan.walk)
-template <int TPB, int WALK>
-__device__ __forceinline__ void k3_infer_run(const DevPlan& plan, const float* __restrict__ feats, size_t row_stride,
-                                             const int64_t* __restrict__ n_records_p, double threshold,
-                                             uint8_t* __restrict__ low_score, float* __restrict__ probs,
-                                             double* __restrict__ qual_out, double* __restrict__ phred_out,
-                                             long long* counts, unsigned chunk_nodes_cap, int phred_mode) {
+// WALK: K3_WALK_* (one kernel per walk, chosen at plan load from plan.walk; the plain walk unless one is named)
+template <int TPB, int WALK = K3_WALK_PLAIN>
+__global__ void __launch_bounds__(TPB, 1)
+k3_infer(const __grid_constant__ DevPlan plan, const float* __restrict__ feats, size_t row_stride,
+         const int64_t* __restrict__ n_records_p, double threshold, uint8_t* __restrict__ low_score,
+         float* __restrict__ probs, double* __restrict__ qual_out, double* __restrict__ phred_out, long long* counts,
+         unsigned chunk_nodes_cap, int phred_mode) {
     extern __shared__ __align__(16) uint8_t smem3[];
     const int F = plan.h.n_features, K = plan.h.n_classes, O = plan.h.n_outputs;
     const unsigned n_trees = plan.h.n_trees;
@@ -1296,28 +1300,6 @@ __device__ __forceinline__ void k3_infer_run(const DevPlan& plan, const float* _
     }
 }
 
-#define K3_INFER_PARAMS                                                                                                 \
-    const __grid_constant__ DevPlan plan, const float* __restrict__ feats, size_t row_stride,                           \
-        const int64_t* __restrict__ n_records_p, double threshold, uint8_t* __restrict__ low_score,                     \
-        float* __restrict__ probs, double* __restrict__ qual_out, double* __restrict__ phred_out, long long* counts,    \
-        unsigned chunk_nodes_cap, int phred_mode
-#define K3_INFER_ARGS \
-    plan, feats, row_stride, n_records_p, threshold, low_score, probs, qual_out, phred_out, counts, chunk_nodes_cap, phred_mode
-template <int TPB>
-__global__ void __launch_bounds__(TPB, 1) k3_infer(K3_INFER_PARAMS) {
-#ifdef UGVC_HOST_EMU
-    // the host emulation's launcher calls k3_infer for every plan: the walk is picked here (on the device, launch_k3 picks
-    // the kernel and this instantiation stays the plain one)
-    if (plan.walk == K3_WALK_CAT) {
-        k3_infer_run<TPB, K3_WALK_CAT>(K3_INFER_ARGS);
-        return;
-    }
-#endif
-    k3_infer_run<TPB, K3_WALK_PLAIN>(K3_INFER_ARGS);
-}
-template <int TPB>
-__global__ void __launch_bounds__(TPB, 1) k3_infer_cat(K3_INFER_PARAMS) { k3_infer_run<TPB, K3_WALK_CAT>(K3_INFER_ARGS); }
-
 #define K3_SMEM_BUDGET (224u * 1024u)
 
 // ------------------------------------------------------------------------------------------
@@ -1406,13 +1388,13 @@ __device__ __forceinline__ void walkhc(const uint8_t* __restrict__ s_node, const
 // completion on an mbarrier) while the current tile is walked, so no warp ever waits on HBM; every thread then turns
 // its own column of the landed slot words into feature values in place (K2's policies) -- a thread only ever reads
 // its own column, so the tile needs no barrier between assembly and walk.
-// k3_heap's body; WALK: K3_WALK_* (one kernel per walk, chosen by the launcher from plan.walk)
-template <int TPB, int NBUF, int NCH, int GROUPS, int WALK>
-__device__ __forceinline__ void
-k3_heap_run(const DevPlan& plan, const uint32_t* __restrict__ raw, const float* __restrict__ feats,
-            size_t row_stride, const int64_t* __restrict__ n_records_p, double threshold, uint8_t* __restrict__ low_score,
-            float* __restrict__ probs, double* __restrict__ qual_out, double* __restrict__ phred_out, long long* counts,
-            unsigned chunk_trees, int phred_mode, unsigned long long* err) {
+// WALK: K3_WALK_* (one kernel per walk, chosen at plan load from plan.walk; the plain walk unless one is named)
+template <int TPB, int NBUF, int NCH, int GROUPS, int WALK = K3_WALK_PLAIN>
+__global__ void __launch_bounds__(TPB, 1)
+k3_heap(const __grid_constant__ DevPlan plan, const uint32_t* __restrict__ raw, const float* __restrict__ feats,
+        size_t row_stride, const int64_t* __restrict__ n_records_p, double threshold, uint8_t* __restrict__ low_score,
+        float* __restrict__ probs, double* __restrict__ qual_out, double* __restrict__ phred_out, long long* counts,
+        unsigned chunk_trees, int phred_mode, unsigned long long* err) {
     extern __shared__ __align__(16) uint8_t smem3[];
     const int F = plan.h.n_features, K = plan.h.n_classes, O = plan.h.n_outputs;
     const unsigned n_trees = plan.h.n_trees;
@@ -1637,52 +1619,41 @@ k3_heap_run(const DevPlan& plan, const uint32_t* __restrict__ raw, const float* 
     }
 }
 
-#define K3_HEAP_PARAMS                                                                                                  \
-    const __grid_constant__ DevPlan plan, const uint32_t* __restrict__ raw, const float* __restrict__ feats,            \
-        size_t row_stride, const int64_t* __restrict__ n_records_p, double threshold, uint8_t* __restrict__ low_score,  \
-        float* __restrict__ probs, double* __restrict__ qual_out, double* __restrict__ phred_out, long long* counts,    \
-        unsigned chunk_trees, int phred_mode, unsigned long long* err
-#define K3_HEAP_ARGS \
-    plan, raw, feats, row_stride, n_records_p, threshold, low_score, probs, qual_out, phred_out, counts, chunk_trees, phred_mode, err
-template <int TPB, int NBUF, int NCH, int GROUPS>
-__global__ void __launch_bounds__(TPB, 1) k3_heap(K3_HEAP_PARAMS) {
-#ifdef UGVC_HOST_EMU
-    // as k3_infer: the host emulation's launcher calls k3_heap for every plan
-    if (plan.walk == K3_WALK_CAT) {
-        k3_heap_run<TPB, NBUF, NCH, GROUPS, K3_WALK_CAT>(K3_HEAP_ARGS);
-        return;
-    }
-#endif
-    k3_heap_run<TPB, NBUF, NCH, GROUPS, K3_WALK_PLAIN>(K3_HEAP_ARGS);
-}
-template <int TPB, int NBUF, int NCH, int GROUPS>
-__global__ void __launch_bounds__(TPB, 1) k3_heap_cat(K3_HEAP_PARAMS) {
-    k3_heap_run<TPB, NBUF, NCH, GROUPS, K3_WALK_CAT>(K3_HEAP_ARGS);
-}
+// ------------------------------------------------------------------------------------------
+// The K3 launch of a plan: kernel, shape, staging, grid and walk (k3_choose, once per plan)
+// ------------------------------------------------------------------------------------------
+// k3_heap's instantiations {tpb, nbuf, nch, groups}, records per tile tpb / groups.  Entries 0-7 are tried in order
+// (UGVC_K3_SHAPE picks one of them): two half-CTAs with one tile each first (most warps for the shared memory), then
+// double-buffered single groups.  Where there are few threads per SM (the tiles are large), sixteen trees per thread
+// in flight make up for it.  Entry 8 is entry 1 walking twelve trees at once (UGVC_K3_NCH448=12).
+struct K3hShape {
+    int tpb, nbuf, nch, groups;
+};
+static constexpr K3hShape K3H_SHAPES[] = {{512, 1, 8, 2},  {448, 1, 8, 2}, {384, 1, 16, 2}, {256, 2, 16, 1}, {192, 2, 16, 1},
+                                          {128, 2, 16, 1}, {256, 1, 8, 1}, {128, 1, 8, 1},  {448, 1, 12, 2}};
+// k3_infer's instantiations: records per CTA, 384 when the feature tile and the whole forest still fit, else 256
+static constexpr int K3I_TPB[] = {384, 256};
 
 // shared-memory plan of k3_heap: records per CTA, tile buffers, trees per staged chunk
 static size_t k3h_tree_bytes(const DevPlan& plan) { return (size_t)(1u << plan.heap_depth) * 10u; }  // 8-byte nodes + leaf rows
-struct K3hShape {
-    int tpb, nbuf, groups;
-};
 static size_t k3_cat_bytes(const DevPlan& plan) { return (size_t)plan.n_cat_words * sizeof(uint32_t); }  // resident
 static size_t k3h_tile_bytes(const DevPlan& plan, K3hShape c) {  // all tile buffers of the CTA + the policy table + bitsets
     return (size_t)c.nbuf * plan.h.n_features * c.tpb * sizeof(float) + (size_t)plan.h.n_features * sizeof(PlanFeature) + 64 +
            k3_cat_bytes(plan);
 }
-static K3hShape k3h_shape(const DevPlan& plan) {
-    static const int force = getenv("UGVC_K3_SHAPE") ? atoi(getenv("UGVC_K3_SHAPE")) : -1;  // profiling knob: index below
+// the K3H_SHAPES entry of a model with a heap form, -1 if none holds it
+static int k3h_shape(const DevPlan& plan) {
+    static const int force = getenv("UGVC_K3_SHAPE") ? atoi(getenv("UGVC_K3_SHAPE")) : -1;  // profiling knob: index 0-7
+    static const int nch448 = getenv("UGVC_K3_NCH448") ? atoi(getenv("UGVC_K3_NCH448")) : 8;  // profiling knob
     const bool forest = plan.h.model_kind != MODEL_LOGISTIC;
     const size_t all = forest ? (size_t)plan.h.n_trees * k3h_tree_bytes(plan) : 0;
-    // two half-CTAs with one tile each first (most warps for the shared memory), then double-buffered single groups
-    const K3hShape cand[8] = {{512, 1, 2}, {448, 1, 2}, {384, 1, 2}, {256, 2, 1}, {192, 2, 1}, {128, 2, 1}, {256, 1, 1}, {128, 1, 1}};
     for (int i = 0; i < 8; ++i) {
         if (force >= 0 && i != force) continue;
-        if (k3h_tile_bytes(plan, cand[i]) + all <= K3_SMEM_BUDGET) return cand[i];
+        if (k3h_tile_bytes(plan, K3H_SHAPES[i]) + all <= K3_SMEM_BUDGET) return i == 1 && nch448 == 12 ? 8 : i;
     }
     for (int i = 3; i < 8; ++i)  // the forest is staged in chunks (single group: the chunks need whole-CTA barriers)
-        if (k3h_tile_bytes(plan, cand[i]) + 16 * k3h_tree_bytes(plan) <= K3_SMEM_BUDGET) return cand[i];
-    return K3hShape{0, 0, 0};
+        if (k3h_tile_bytes(plan, K3H_SHAPES[i]) + 16 * k3h_tree_bytes(plan) <= K3_SMEM_BUDGET) return i;
+    return -1;
 }
 static unsigned k3h_chunk_trees(const DevPlan& plan, K3hShape sh) {
     if (plan.h.model_kind == MODEL_LOGISTIC) return 0;
@@ -1692,22 +1663,17 @@ static unsigned k3h_chunk_trees(const DevPlan& plan, K3hShape sh) {
     if (n < plan.h.n_trees) n &= ~(size_t)15;  // whole groups of chains
     return (unsigned)n;
 }
-bool k3_fused_available(const DevPlan& plan) {
-    if (plan.h.model_kind == MODEL_NONE) return false;
-    if (plan.h.model_kind != MODEL_LOGISTIC && plan.heap_depth == 0) return false;
-    return k3h_shape(plan).tpb != 0;
-}
-K3Config k3_heap_config(const DevPlan& plan, int sm_count) {
-    const K3hShape sh = k3h_shape(plan);
+// k3_heap's launch for a model with a heap form; shape -1 (and nothing else set) when no shape holds the model
+static K3Config k3_heap_config(const DevPlan& plan, int sm_count) {
     K3Config c{};
     c.kernel = K3_KERNEL_HEAP;
+    c.shape = k3h_shape(plan);
+    if (c.shape < 0) return c;
+    const K3hShape sh = K3H_SHAPES[c.shape];
     c.tpb = sh.tpb;
     c.nbuf = sh.nbuf;
     c.groups = sh.groups;
-    // few threads per SM (the tiles are large): sixteen trees per thread in flight make up for it
-    static const int nch448 = getenv("UGVC_K3_NCH448") ? atoi(getenv("UGVC_K3_NCH448")) : 8;  // profiling knob
-    if (sh.groups == 2) c.nch = sh.tpb == 512 ? 8 : sh.tpb == 448 ? (nch448 == 12 ? 12 : 8) : 16;
-    else c.nch = sh.nbuf == 2 ? 16 : 8;
+    c.nch = sh.nch;
     c.chunk = k3h_chunk_trees(plan, sh);
     c.resident = plan.h.model_kind == MODEL_LOGISTIC || c.chunk >= plan.h.n_trees;
     c.smem = k3h_tile_bytes(plan, sh) + (size_t)c.chunk * k3h_tree_bytes(plan);
@@ -1718,48 +1684,21 @@ K3Config k3_heap_config(const DevPlan& plan, int sm_count) {
     c.walk = (int)plan.walk;
     return c;
 }
-#ifndef UGVC_HOST_EMU
-void launch_k3_fused(const DevPlan& plan, const uint32_t* raw, const float* feats, size_t row_stride,
-                     const int64_t* d_n_records, double threshold, uint8_t* low_score, float* probs, double* qual,
-                     double* phreds, int phred_mode, long long* d_counts, unsigned long long* d_err, int sm_count,
-                     cudaStream_t st) {
-    const K3Config c = k3_heap_config(plan, sm_count);
-#define K3H_LAUNCH(T, B, C, G)                                                                                             \
-    do {                                                                                                                   \
-        if (plan.walk == K3_WALK_CAT)                                                                                      \
-            k3_heap_cat<T, B, C, G><<<c.grid, T, c.smem, st>>>(plan, raw, feats, row_stride, d_n_records, threshold,        \
-                                                               low_score, probs, qual, phreds, d_counts, c.chunk,           \
-                                                               phred_mode, d_err);                                          \
-        else                                                                                                               \
-            k3_heap<T, B, C, G><<<c.grid, T, c.smem, st>>>(plan, raw, feats, row_stride, d_n_records, threshold, low_score, \
-                                                           probs, qual, phreds, d_counts, c.chunk, phred_mode, d_err);      \
-    } while (0)
-    if (c.groups == 2 && c.tpb == 512) K3H_LAUNCH(512, 1, 8, 2);
-    else if (c.groups == 2 && c.tpb == 448 && c.nch == 12) K3H_LAUNCH(448, 1, 12, 2);
-    else if (c.groups == 2 && c.tpb == 448) K3H_LAUNCH(448, 1, 8, 2);
-    else if (c.groups == 2) K3H_LAUNCH(384, 1, 16, 2);
-    else if (c.tpb == 256 && c.nbuf == 2) K3H_LAUNCH(256, 2, 16, 1);
-    else if (c.tpb == 192) K3H_LAUNCH(192, 2, 16, 1);
-    else if (c.tpb == 256) K3H_LAUNCH(256, 1, 8, 1);
-    else if (c.nbuf == 2) K3H_LAUNCH(128, 2, 16, 1);
-    else K3H_LAUNCH(128, 1, 8, 1);
-#undef K3H_LAUNCH
-}
-#endif
+
 static size_t k3_forest_bytes(const DevPlan& plan) {
     if (plan.h.model_kind == MODEL_LOGISTIC || plan.h.model_kind == MODEL_NONE) return 0;
     return (size_t)plan.h.n_nodes * sizeof(uint2);
 }
 static size_t k3_roots_bytes(const DevPlan& plan) { return ((size_t)plan.h.n_trees + 2) * sizeof(uint32_t); }
-// records per CTA: 384 when the feature tile and the whole forest still fit, else 256
-static int k3_tpb(const DevPlan& plan) {
+// the K3I_TPB entry of a model
+static int k3i_shape(const DevPlan& plan) {
     const size_t forest = k3_forest_bytes(plan);
-    if (forest == 0) return 256;
-    const size_t need384 = (size_t)plan.h.n_features * 384 * sizeof(float) + forest + k3_roots_bytes(plan) + k3_cat_bytes(plan);
-    static const int force = getenv("UGVC_K3_TPB") ? atoi(getenv("UGVC_K3_TPB")) : 0;  // profiling knob
-    if (force == 256 || force == 384) return force == 384 && need384 > K3_SMEM_BUDGET ? 256 : force;
-    return need384 <= K3_SMEM_BUDGET ? 384 : 256;
+    if (forest == 0) return 1;
+    const size_t need384 = (size_t)plan.h.n_features * K3I_TPB[0] * sizeof(float) + forest + k3_roots_bytes(plan) + k3_cat_bytes(plan);
+    static const int force = getenv("UGVC_K3_TPB") ? atoi(getenv("UGVC_K3_TPB")) : 0;  // profiling knob: 256, or 384 where it fits
+    return force != 256 && need384 <= K3_SMEM_BUDGET ? 0 : 1;
 }
+static int k3_tpb(const DevPlan& plan) { return K3I_TPB[k3i_shape(plan)]; }
 // nodes the shared-memory forest buffer holds (0 for linear models)
 static unsigned k3_chunk_nodes(const DevPlan& plan) {
     if (k3_forest_bytes(plan) == 0) return 0;
@@ -1769,27 +1708,27 @@ static unsigned k3_chunk_nodes(const DevPlan& plan) {
     const size_t room = (K3_SMEM_BUDGET - tile - roots) / sizeof(uint2);
     return (unsigned)(room < plan.h.n_nodes ? room : plan.h.n_nodes);
 }
-size_t k3_smem_bytes(const DevPlan& plan) {
+static size_t k3_smem_bytes(const DevPlan& plan) {
     size_t b = (size_t)plan.h.n_features * k3_tpb(plan) * sizeof(float);
     const unsigned cap = k3_chunk_nodes(plan);
     if (cap) b += (size_t)cap * sizeof(uint2) + k3_roots_bytes(plan) + k3_cat_bytes(plan);
     return b;
 }
-unsigned k3_chunk_nodes_cap(const DevPlan& plan) { return k3_chunk_nodes(plan); }
-bool k3_plan_fits(const DevPlan& plan) {
+static bool k3_plan_fits(const DevPlan& plan) {
     if (k3_forest_bytes(plan) == 0) return (size_t)plan.h.n_features * 256 * sizeof(float) <= K3_SMEM_BUDGET;
     return k3_chunk_nodes(plan) > 0;
 }
 // most features k3_infer holds for this model: a 256-record tile, plus for a forest the tree roots, the category
 // bitsets and 4 KiB of nodes
-unsigned k3_infer_max_features(const DevPlan& plan) {
+static unsigned k3_infer_max_features(const DevPlan& plan) {
     const size_t fixed = k3_forest_bytes(plan) ? k3_roots_bytes(plan) + k3_cat_bytes(plan) + 4096 : 0;
     return fixed >= K3_SMEM_BUDGET ? 0u : (unsigned)((K3_SMEM_BUDGET - fixed) / (256 * sizeof(float)));
 }
-K3Config k3_infer_config(const DevPlan& plan, int sm_count) {
+static K3Config k3_infer_config(const DevPlan& plan, int sm_count) {
     K3Config c{};
     c.kernel = K3_KERNEL_INFER;
-    c.tpb = k3_tpb(plan);
+    c.shape = k3i_shape(plan);
+    c.tpb = K3I_TPB[c.shape];
     c.nbuf = c.groups = 1;
     c.nch = K3_CHAINS;
     c.chunk = k3_chunk_nodes(plan);
@@ -1803,19 +1742,66 @@ K3Config k3_infer_config(const DevPlan& plan, int sm_count) {
     return c;
 }
 
+bool k3_choose(const DevPlan& plan, const uint32_t* tree_root, int sm_count, K3Config* out, std::string* why) {
+    // UGVC_K3_LEGACY=1 (profiling): K2 + k3_infer even where k3_heap would run
+    static const bool legacy = getenv("UGVC_K3_LEGACY") && *getenv("UGVC_K3_LEGACY") != '0';
+    // k3_heap (K2 fused into its tile load) when the model has a heap form: it holds every plan the compiler makes (up
+    // to 250 features)
+    if (!legacy && (plan.h.model_kind == MODEL_LOGISTIC || plan.heap_depth != 0)) {
+        const K3Config c = k3_heap_config(plan, sm_count);
+        if (c.shape >= 0) {
+            *out = c;
+            return true;
+        }
+    }
+    // else K2 + k3_infer, which holds fewer features
+    if (!k3_plan_fits(plan)) {
+        *why = std::string("plan needs more shared memory than one sm_90 CTA has: k3_infer (") +
+               (legacy ? "selected by UGVC_K3_LEGACY" : "forests deeper than 8 or with 65536 leaf rows or more") +
+               ") holds at most " + std::to_string(k3_infer_max_features(plan)) + " features for this model, it has " +
+               std::to_string(plan.h.n_features);
+        return false;
+    }
+    if (plan.h.model_kind != MODEL_LOGISTIC) {
+        const unsigned cap = k3_chunk_nodes(plan);
+        for (uint32_t t = 0; t < plan.h.n_trees; ++t)
+            if (tree_root[t + 1] - tree_root[t] > cap) {
+                *why = "a single tree does not fit k3_infer's shared-memory forest buffer";
+                return false;
+            }
+    }
+    *out = k3_infer_config(plan, sm_count);
+    return true;
+}
+
 #ifndef UGVC_HOST_EMU
-void launch_k3(const DevPlan& plan, const float* feats, size_t row_stride, const int64_t* d_n_records,
-               double threshold, uint8_t* low_score, float* probs, double* qual, double* phreds, int phred_mode,
-               long long* d_counts, int sm_count, cudaStream_t st) {
-    const K3Config c = k3_infer_config(plan, sm_count);
-#define K3I_LAUNCH(K, T) \
-    K<T><<<c.grid, T, c.smem, st>>>(plan, feats, row_stride, d_n_records, threshold, low_score, probs, qual, phreds, d_counts, \
-                                   c.chunk, phred_mode)
-    if (plan.walk == K3_WALK_CAT && c.tpb == 384) K3I_LAUNCH(k3_infer_cat, 384);
-    else if (plan.walk == K3_WALK_CAT) K3I_LAUNCH(k3_infer_cat, 256);
-    else if (c.tpb == 384) K3I_LAUNCH(k3_infer, 384);
-    else K3I_LAUNCH(k3_infer, 256);
-#undef K3I_LAUNCH
+// the instantiations of one walk, in table order
+template <int WALK, size_t... S>
+static auto k3h_kernels(std::index_sequence<S...>) {
+    return std::array{&k3_heap<K3H_SHAPES[S].tpb, K3H_SHAPES[S].nbuf, K3H_SHAPES[S].nch, K3H_SHAPES[S].groups, WALK>...};
+}
+template <int WALK, size_t... S>
+static auto k3i_kernels(std::index_sequence<S...>) {
+    return std::array{&k3_infer<K3I_TPB[S], WALK>...};
+}
+// [walk][K3Config::shape]
+static const auto K3H_KERNELS = std::array{k3h_kernels<K3_WALK_PLAIN>(std::make_index_sequence<std::size(K3H_SHAPES)>()),
+                                           k3h_kernels<K3_WALK_CAT>(std::make_index_sequence<std::size(K3H_SHAPES)>())};
+static const auto K3I_KERNELS = std::array{k3i_kernels<K3_WALK_PLAIN>(std::make_index_sequence<std::size(K3I_TPB)>()),
+                                           k3i_kernels<K3_WALK_CAT>(std::make_index_sequence<std::size(K3I_TPB)>())};
+
+void launch_k3(const DevPlan& plan, const K3Config& c, const uint32_t* raw, const float* feats, size_t row_stride,
+               const int64_t* d_n_records, double threshold, uint8_t* low_score, float* probs, double* qual,
+               double* phreds, int phred_mode, long long* d_counts, unsigned long long* d_err, cudaStream_t st) {
+    if (c.kernel == K3_KERNEL_HEAP) {
+        const auto k = K3H_KERNELS[c.walk][c.shape];
+        k<<<c.grid, c.tpb, c.smem, st>>>(plan, raw, feats, row_stride, d_n_records, threshold, low_score, probs, qual, phreds,
+                                         d_counts, c.chunk, phred_mode, d_err);
+    } else {
+        const auto k = K3I_KERNELS[c.walk][c.shape];
+        k<<<c.grid, c.tpb, c.smem, st>>>(plan, feats, row_stride, d_n_records, threshold, low_score, probs, qual, phreds,
+                                         d_counts, c.chunk, phred_mode);
+    }
 }
 
 cudaError_t kernels_configure(const DevPlan& plan) {
@@ -1832,33 +1818,33 @@ cudaError_t kernels_configure(const DevPlan& plan) {
     e = cudaFuncSetAttribute(k1_parse_frame, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k1_smem_bytes(plan));
     if (e != cudaSuccess) return e;
 #endif
-    {
-        const int lim = 226 * 1024;  // a few static bytes (the mbarrier words) come on top of the dynamic part
-        if ((e = cudaFuncSetAttribute(k3_heap<512, 1, 8, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim)) != cudaSuccess) return e;
-        if ((e = cudaFuncSetAttribute(k3_heap<384, 1, 16, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim)) != cudaSuccess) return e;
-        if ((e = cudaFuncSetAttribute(k3_heap<448, 1, 8, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim)) != cudaSuccess) return e;
-        if ((e = cudaFuncSetAttribute(k3_heap<448, 1, 12, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim)) != cudaSuccess) return e;
-        if ((e = cudaFuncSetAttribute(k3_heap<256, 2, 16, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim)) != cudaSuccess) return e;
-        if ((e = cudaFuncSetAttribute(k3_heap<192, 2, 16, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim)) != cudaSuccess) return e;
-        if ((e = cudaFuncSetAttribute(k3_heap<256, 1, 8, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim)) != cudaSuccess) return e;
-        if ((e = cudaFuncSetAttribute(k3_heap<128, 2, 16, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim)) != cudaSuccess) return e;
-        if ((e = cudaFuncSetAttribute(k3_heap<128, 1, 8, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim)) != cudaSuccess) return e;
-        if ((e = cudaFuncSetAttribute(k3_heap_cat<512, 1, 8, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim)) != cudaSuccess) return e;
-        if ((e = cudaFuncSetAttribute(k3_heap_cat<384, 1, 16, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim)) != cudaSuccess) return e;
-        if ((e = cudaFuncSetAttribute(k3_heap_cat<448, 1, 8, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim)) != cudaSuccess) return e;
-        if ((e = cudaFuncSetAttribute(k3_heap_cat<448, 1, 12, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim)) != cudaSuccess) return e;
-        if ((e = cudaFuncSetAttribute(k3_heap_cat<256, 2, 16, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim)) != cudaSuccess) return e;
-        if ((e = cudaFuncSetAttribute(k3_heap_cat<192, 2, 16, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim)) != cudaSuccess) return e;
-        if ((e = cudaFuncSetAttribute(k3_heap_cat<256, 1, 8, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim)) != cudaSuccess) return e;
-        if ((e = cudaFuncSetAttribute(k3_heap_cat<128, 2, 16, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim)) != cudaSuccess) return e;
-        if ((e = cudaFuncSetAttribute(k3_heap_cat<128, 1, 8, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim)) != cudaSuccess) return e;
+    for (const auto& walk : K3H_KERNELS)  // a few static bytes (the mbarrier words) come on top of the dynamic part
+        for (const auto k : walk)
+            if ((e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024)) != cudaSuccess) return e;
+    for (const auto& walk : K3I_KERNELS)
+        for (const auto k : walk)
+            if ((e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)) != cudaSuccess) return e;
+    return cudaSuccess;
+}
+#else
+// host emulation (tests/host_emu): the chosen kernel and walk with one thread per CTA and the product's chunk, so a
+// forest larger than it runs the chunk loop here too.  smem3 is the emulation's shared memory.
+void launch_k3(const DevPlan& plan, const K3Config& c, const uint32_t* raw, const float* feats, size_t row_stride,
+               const int64_t* d_n_records, double threshold, uint8_t* low_score, float* probs, double* qual,
+               double* phreds, int phred_mode, long long* d_counts, unsigned long long* d_err, cudaStream_t) {
+    threadIdx = blockIdx = dim3(0, 0, 0);
+    blockDim = gridDim = dim3(1, 1, 1);
+    if (c.smem > sizeof(smem3)) {  // c.smem is sized for the product's tile, wider than the emulated one
+        fprintf(stderr, "host_emu: K3 does not fit the emulated shared memory\n");
+        abort();
     }
-    e = cudaFuncSetAttribute(k3_infer<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
-    if (e != cudaSuccess) return e;
-    e = cudaFuncSetAttribute(k3_infer_cat<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
-    if (e != cudaSuccess) return e;
-    e = cudaFuncSetAttribute(k3_infer_cat<384>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
-    if (e != cudaSuccess) return e;
-    return cudaFuncSetAttribute(k3_infer<384>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
+    const bool cat = c.walk == K3_WALK_CAT;
+    if (c.kernel == K3_KERNEL_HEAP)
+        (cat ? k3_heap<1, 1, 8, 1, K3_WALK_CAT> : k3_heap<1, 1, 8, 1, K3_WALK_PLAIN>)(
+            plan, raw, feats, row_stride, d_n_records, threshold, low_score, probs, qual, phreds, d_counts, c.chunk,
+            phred_mode, d_err);
+    else
+        (cat ? k3_infer<1, K3_WALK_CAT> : k3_infer<1, K3_WALK_PLAIN>)(
+            plan, feats, row_stride, d_n_records, threshold, low_score, probs, qual, phreds, d_counts, c.chunk, phred_mode);
 }
 #endif  // !UGVC_HOST_EMU

@@ -3,6 +3,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <string>
+
 #include "../../include/ugvc_b200.h"
 #include "plan.h"
 
@@ -178,24 +180,15 @@ void launch_k1(const DevPlan& plan, const DevSchedule& sched, const uint8_t* d_t
                long long* d_counts, int sm_count, cudaStream_t st);
 void launch_k2(const DevPlan& plan, const uint32_t* raw, size_t row_stride, const int64_t* d_n_records, float* feats,
                unsigned long long* d_err, int sm_count, cudaStream_t st);
-void launch_k3(const DevPlan& plan, const float* feats, size_t row_stride, const int64_t* d_n_records,
-               double threshold, uint8_t* low_score, float* probs, double* qual, double* phreds, int phred_mode,
-               long long* d_counts, int sm_count, cudaStream_t st);
-// K2 + K3 in one kernel: the feature tile is assembled from the raw slots (or taken from a dense feature
-// matrix when raw is NULL) while it is staged; false when the plan's model has no heap form (then K2 + launch_k3)
-bool k3_fused_available(const DevPlan& plan);
-void launch_k3_fused(const DevPlan& plan, const uint32_t* raw, const float* feats, size_t row_stride,
-                     const int64_t* d_n_records, double threshold, uint8_t* low_score, float* probs, double* qual,
-                     double* phreds, int phred_mode, long long* d_counts, unsigned long long* d_err, int sm_count,
-                     cudaStream_t st);
 void launch_k1_fast(const DevPlan& plan, const DevFast& fast, const DevSchedule& sched, const uint8_t* d_text, size_t n_bytes,
                     uint32_t* scratch, int64_t* line_start, size_t cap_records, int64_t* d_n_records, uint32_t* raw,
                     size_t row_stride, ugvc_recinfo* recinfo, uint32_t* slow_list, unsigned long long* d_err,
                     long long* d_counts, int sm_count, cudaStream_t st);
-// The K3 launch of a plan, as launch_k3_fused (k3_heap) / launch_k3 (k3_infer) make it; ugvc_test_k3_config reports it
+// The K3 launch of a plan; ugvc_test_k3_config reports it
 enum { K3_KERNEL_HEAP = 0, K3_KERNEL_INFER = 1 };
 struct K3Config {
     int kernel;             // K3_KERNEL_HEAP / K3_KERNEL_INFER
+    int shape;              // the kernel's instantiation: index into kernels.cu's K3H_SHAPES / K3I_TPB
     int tpb, nbuf, groups;  // threads per CTA, tile buffers per group, independent groups per CTA (records per tile: tpb / groups)
     int nch;                // trees one thread walks at once
     unsigned chunk;         // k3_heap: trees per staged forest chunk; k3_infer: nodes the forest buffer holds (0: linear model)
@@ -204,11 +197,13 @@ struct K3Config {
     int grid;               // CTAs of the persistent grid
     int walk;               // K3_WALK_* of the instantiation that runs
 };
-K3Config k3_heap_config(const DevPlan& plan, int sm_count);   // only when k3_fused_available(plan)
-K3Config k3_infer_config(const DevPlan& plan, int sm_count);
+// The K3 launch of a plan with a model: k3_heap, which assembles the features from K1's raw slots in its tile load,
+// when the model has a heap form, else K2 + k3_infer.  tree_root: the host copy of plan.tree_root.  False, with the
+// reason in *why, when neither kernel holds the plan.
+bool k3_choose(const DevPlan& plan, const uint32_t* tree_root, int sm_count, K3Config* out, std::string* why);
+// K3 as c says.  k3_heap reads the raw slots, or the dense feature matrix feats when raw is NULL; k3_infer reads feats.
+void launch_k3(const DevPlan& plan, const K3Config& c, const uint32_t* raw, const float* feats, size_t row_stride,
+               const int64_t* d_n_records, double threshold, uint8_t* low_score, float* probs, double* qual,
+               double* phreds, int phred_mode, long long* d_counts, unsigned long long* d_err, cudaStream_t st);
 size_t k1_smem_bytes(const DevPlan& plan);
-size_t k3_smem_bytes(const DevPlan& plan);
-bool k3_plan_fits(const DevPlan& plan);
-unsigned k3_chunk_nodes_cap(const DevPlan& plan);
-unsigned k3_infer_max_features(const DevPlan& plan);
 cudaError_t kernels_configure(const DevPlan& plan);
