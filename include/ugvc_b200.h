@@ -382,6 +382,16 @@ int ugvc_ma_merge(ugvc_ma* h, const double* lik, int64_t n_rows, int n_classes, 
 /* Test hook: K3's xgboost-flavoured fp32 sigmoid evaluated on the device for an array of margins (p1 and the
  * exponential it used). */
 int ugvc_test_device_sigmoid(ugvc_ctx* ctx, const float* margins, int n, float* out_p1, float* out_e);
+/* Test hook: the record writer's "%g" (csrc/fileio.cu: fio_format_g) on the device for n float32 values.  out receives
+ * 16 bytes per value, the slot layout of the writer: the text in bytes 0..14 (zero padded), its length in byte 15;
+ * length 0 = a value the device writer leaves to the host writer (exponent form, negative, inf, NaN). */
+int ugvc_test_format_g(ugvc_ctx* ctx, const float* v, int64_t n, uint8_t* out);
+/* Test hook: the BGZF encoder of ugvc_filter_bgzf (deflate, block offsets, pack) on the caller's n bytes, staged in
+ * lane 0's writer buffer (needs ugvc_reserve; n at most what that buffer holds).  encoder 0 = one warp per block (the
+ * default), 1 = one thread per block (UGVC_DEFLATE_THREADS=1).  out receives the packed blocks (*out_bytes bytes),
+ * out_block_csize the size of each of the *out_n_blocks blocks of 57344 input bytes (none for n = 0). */
+int ugvc_test_device_deflate(ugvc_ctx* ctx, const uint8_t* data, size_t n, int encoder, uint8_t* out, size_t capacity,
+                             uint32_t* out_block_csize, size_t block_capacity, size_t* out_bytes, size_t* out_n_blocks);
 /* Test hook: the K3 launch the loaded plan gets (also in the host emulation, which runs the same chunking).
  * out = {kernel (0 k3_heap, 1 k3_infer), threads per CTA, tile buffers per group, groups per CTA (records per tile:
  * threads / groups), trees one thread walks at once, forest chunk (k3_heap: trees, k3_infer: nodes; 0 for a linear

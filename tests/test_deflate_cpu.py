@@ -68,6 +68,20 @@ def test_edge_inputs():
              rng.integers(0, 256, size=1000, dtype=np.uint8).tobytes(),
              (b"chr1\t12345\t.\tA\tG\t50\tPASS\tAC=1;AF=0.5\n" * 2000)[:CHUNK],
              b"\xff" * 70 + b"\x00" * 70 + b"\xff" * 700]
+    # short periods: matches overlap their own source, one match covers whole 32-position windows
+    for p in (2, 3, 31, 32, 33):
+        cases.append((rng.integers(0, 256, size=p, dtype=np.uint8).tobytes() * (CHUNK // p + 1))[:CHUNK])
+    # a chunk repeated exactly 32768 bytes later (the largest distance DEFLATE allows) and 32769 bytes later (beyond)
+    for period in (32768, 32769):
+        unit = rng.integers(0, 256, size=256, dtype=np.uint8).tobytes() + b"\0" * (period - 256)
+        cases.append((unit * 2)[:CHUNK])
+    # bytes >= 0x90 take 9-bit literal codes: stored when random, compressed when drawn from a vocabulary
+    cases.append(rng.integers(0x90, 0x100, size=CHUNK, dtype=np.uint8).tobytes())
+    words = [rng.integers(0x90, 0x100, size=int(rng.integers(3, 40)), dtype=np.uint8).tobytes() for _ in range(64)]
+    cases.append(b"".join(words[int(k)] for k in rng.integers(0, 64, size=3000))[:CHUNK])
+    # runs around the longest match (258) between random bytes
+    for r in (257, 258, 259, 260):
+        cases.append(b"".join(rng.integers(0, 256, size=20, dtype=np.uint8).tobytes() + b"R" * r for _ in range(50)))
     for data in cases:
         check_block(encode(L, data), data)
 

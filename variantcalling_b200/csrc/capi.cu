@@ -1233,6 +1233,10 @@ extern "C" int ugvc_filter_bgzf(ugvc_ctx* ctx, int, const uint8_t*, size_t, uint
 }
 extern "C" int ugvc_filter_bgzf_stage_ms(ugvc_ctx*, int, float*) { return UGVC_E_STATE; }
 extern "C" int ugvc_filter_bgzf_first_records(ugvc_ctx*, int, const uint64_t*, int, int64_t*) { return UGVC_E_STATE; }
+extern "C" int ugvc_test_device_deflate(ugvc_ctx* ctx, const uint8_t*, size_t, int, uint8_t*, size_t, uint32_t*, size_t, size_t*,
+                                        size_t*) {
+    return fail(ctx, UGVC_E_STATE, "the device BGZF encoder is not part of the host emulation");
+}
 #else
 static int file_bufs(ugvc_ctx* ctx, Lane& l) {
     Lane::FileBufs& f = l.fb;
@@ -1267,6 +1271,31 @@ static int file_bufs(ugvc_ctx* ctx, Lane& l) {
         CU(cudaMemcpy(ctx->d_def_tables, t, sizeof(DefTables), cudaMemcpyHostToDevice));
         delete t;
     }
+    return UGVC_OK;
+}
+
+// UGVC_DEFLATE_THREADS=1: the thread-per-block encoder instead of the warp-per-block one (A/B)
+static int deflate_encoder() {
+    static const int enc = [] {
+        const char* e = getenv("UGVC_DEFLATE_THREADS");
+        return e && e[0] == '1' ? FIO_ENC_THREAD : FIO_ENC_WARP;
+    }();
+    return enc;
+}
+
+// The encoder of the file path: f.d_out_text[0, n_text) (16 zero bytes after it: the encoder reads whole words) ->
+// n_blocks BGZF blocks (deflate), their sizes widened and scanned into offsets, the blocks packed back to back into
+// f.d_packed.  The sizes stay in f.d_bsize.
+static int encode_blocks(ugvc_ctx* ctx, Lane::FileBufs& f, size_t n_text, int n_blocks, int encoder, cudaStream_t st) {
+    CU(cudaGetLastError());
+    CU(fio_launch_deflate(f.d_out_text, n_text, ctx->d_def_tables, f.d_blocks, f.d_bsize, n_blocks, encoder, st));
+    fio_launch_widen(f.d_bsize, f.d_bwide, n_blocks, st);
+    CU(cudaGetLastError());
+    CU(cudaMemsetAsync(f.d_bwide + n_blocks, 0, sizeof(uint64_t), st));
+    size_t tmp = f.scan_tmp_bytes;
+    CU(fio_scan_u64(f.d_scan_tmp, tmp, f.d_bwide, f.d_boff, n_blocks + 1, st));
+    fio_launch_pack(f.d_blocks, f.d_bsize, f.d_bwide, f.d_boff, n_blocks, f.d_packed, ctx->sm_count, st);
+    CU(cudaGetLastError());
     return UGVC_OK;
 }
 
@@ -1340,15 +1369,8 @@ extern "C" int ugvc_filter_bgzf(ugvc_ctx* ctx, int lane, const uint8_t* bgzf, si
     const int n_blocks = (int)((out_text + DEF_CHUNK - 1) / DEF_CHUNK);
     if ((size_t)n_blocks > f.cap_blocks || (out_block_csize && (size_t)n_blocks > block_capacity))
         return fail(ctx, UGVC_E_ARG, "filter_bgzf: more output blocks than room for them");
-    CU(cudaGetLastError());
-    CU(fio_launch_deflate(f.d_out_text, out_text, ctx->d_def_tables, f.d_blocks, f.d_bsize, n_blocks, st));
-    fio_launch_widen(f.d_bsize, f.d_bwide, n_blocks, st);
-    CU(cudaGetLastError());
-    CU(cudaMemsetAsync(f.d_bwide + n_blocks, 0, sizeof(uint64_t), st));
-    tmp = f.scan_tmp_bytes;
-    CU(fio_scan_u64(f.d_scan_tmp, tmp, f.d_bwide, f.d_boff, n_blocks + 1, st));
-    fio_launch_pack(f.d_blocks, f.d_bsize, f.d_bwide, f.d_boff, n_blocks, f.d_packed, ctx->sm_count, st);
-    CU(cudaGetLastError());
+    rc = encode_blocks(ctx, f, out_text, n_blocks, deflate_encoder(), st);
+    if (rc) return rc;
     f.h_bsize.resize((size_t)n_blocks + 1);
     if (n_blocks) CU(cudaMemcpyAsync(f.h_bsize.data(), f.d_bsize, (size_t)n_blocks * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
     CU(cudaEventRecord(f.ev[4], st));
@@ -1392,6 +1414,43 @@ extern "C" int ugvc_filter_bgzf_first_records(ugvc_ctx* ctx, int lane, const uin
     fio_launch_first_records(l.b.line_start, l.last_n, d_off, n, d_out, l.stream);
     CU(cudaMemcpyAsync(out_first_record, d_out, (size_t)n * sizeof(int64_t), cudaMemcpyDeviceToHost, l.stream));
     CU(cudaStreamSynchronize(l.stream));
+    return UGVC_OK;
+}
+
+extern "C" int ugvc_test_device_deflate(ugvc_ctx* ctx, const uint8_t* data, size_t n, int encoder, uint8_t* out, size_t capacity,
+                                        uint32_t* out_block_csize, size_t block_capacity, size_t* out_bytes, size_t* out_n_blocks) {
+    // test hook: the file path's encoder (encode_blocks) on the caller's bytes, staged in lane 0's writer buffer the way
+    // ugvc_filter_bgzf stages the edited text
+    if (!ctx || (n && !data) || !out_bytes || !out_n_blocks || (encoder != FIO_ENC_WARP && encoder != FIO_ENC_THREAD))
+        return UGVC_E_ARG;
+    if (ctx->lanes.empty()) return fail(ctx, UGVC_E_STATE, "test_device_deflate: reserve first (the bytes go to lane 0)");
+    CU(cudaSetDevice(ctx->device));
+    Lane& l = ctx->lanes[0];
+    if (l.submitted) return fail(ctx, UGVC_E_STATE, "test_device_deflate: lane 0 has a batch in flight");
+    int rc = file_bufs(ctx, l);
+    if (rc) return rc;
+    Lane::FileBufs& f = l.fb;
+    if (n > f.cap_out) return fail(ctx, UGVC_E_ARG, "test_device_deflate: more bytes than the writer's buffer holds");
+    const int n_blocks = (int)((n + DEF_CHUNK - 1) / DEF_CHUNK);
+    if ((size_t)n_blocks > block_capacity || (n_blocks && !out_block_csize))
+        return fail(ctx, UGVC_E_ARG, "test_device_deflate: more output blocks than room for them");
+    cudaStream_t st = l.stream;
+    (void)cudaGetLastError();
+    if (n) CU(cudaMemcpyAsync(f.d_out_text, data, n, cudaMemcpyHostToDevice, st));
+    CU(cudaMemsetAsync(f.d_out_text + n, 0, 16, st));
+    rc = encode_blocks(ctx, f, n, n_blocks, encoder, st);
+    if (rc) return rc;
+    f.h_bsize.resize((size_t)n_blocks + 1);
+    if (n_blocks) CU(cudaMemcpyAsync(f.h_bsize.data(), f.d_bsize, (size_t)n_blocks * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    size_t packed = 0;
+    for (int b = 0; b < n_blocks; ++b) packed += f.h_bsize[b];
+    if (packed > capacity || (packed && !out)) return fail(ctx, UGVC_E_ARG, "test_device_deflate: capacity smaller than the compressed output");
+    if (packed) CU(cudaMemcpyAsync(out, f.d_packed, packed, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    if (n_blocks) memcpy(out_block_csize, f.h_bsize.data(), (size_t)n_blocks * sizeof(uint32_t));
+    *out_bytes = packed;
+    *out_n_blocks = (size_t)n_blocks;
     return UGVC_OK;
 }
 #endif  // !UGVC_HOST_EMU
@@ -1564,8 +1623,26 @@ extern "C" int ugvc_test_device_sigmoid(ugvc_ctx* ctx, const float* margins, int
     cudaFree(d_e);
     return UGVC_OK;
 }
+extern "C" int ugvc_test_format_g(ugvc_ctx* ctx, const float* v, int64_t n, uint8_t* out) {
+    // test hook: the record writer's "%g" (fileio.cu: fio_format_g) on the device, for comparison with a correctly
+    // rounded formatter; 16 bytes per value as splice_len stores them
+    if (!ctx || !v || !out || n <= 0) return UGVC_E_ARG;
+    CU(cudaSetDevice(ctx->device));
+    float* d_v = nullptr;
+    uint8_t* d_out = nullptr;
+    CU(cudaMalloc(&d_v, (size_t)n * sizeof(float)));
+    CU(cudaMalloc(&d_out, (size_t)n * 16));
+    CU(cudaMemcpy(d_v, v, (size_t)n * sizeof(float), cudaMemcpyHostToDevice));
+    fio_launch_test_format_g(d_v, n, d_out, ctx->sm_count, nullptr);
+    CU(cudaGetLastError());
+    CU(cudaMemcpy(out, d_out, (size_t)n * 16, cudaMemcpyDeviceToHost));
+    cudaFree(d_v);
+    cudaFree(d_out);
+    return UGVC_OK;
+}
 #else
 extern "C" int ugvc_test_device_sigmoid(ugvc_ctx*, const float*, int, float*, float*) { return UGVC_E_CUDA; }
+extern "C" int ugvc_test_format_g(ugvc_ctx*, const float*, int64_t, uint8_t*) { return UGVC_E_CUDA; }
 #endif
 
 extern "C" int ugvc_test_k3_config(ugvc_ctx* ctx, int32_t out[9]) {

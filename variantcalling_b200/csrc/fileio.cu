@@ -14,7 +14,6 @@
 // Same text as the host writer produces (tests compare the two), so the output contract is unchanged.
 #include <cuda_runtime.h>
 #include <stdint.h>
-#include <stdlib.h>
 
 #include <cub/device/device_scan.cuh>
 
@@ -22,45 +21,46 @@
 #include "fileio.cuh"
 
 // ---- "%g" of a float32 >= 0 (what htslib prints for INFO / QUAL floats): six significant digits, exact
-// round-half-even on the binary value, trailing zeros dropped.  Values that need the exponent form return 0.
+// round-half-even on the binary value, trailing zeros dropped.  Values that need the exponent form return 0.  %g
+// picks the form from the exponent of the value ROUNDED to six digits: 9.999995e-5 prints as 0.0001, 999999.5 as 1e+06.
 __device__ int fio_format_g(float v, char* out) {
     if (v == 0.0f) {
         out[0] = '0';
         return 1;
     }
-    if (!(v >= 1e-4f && v < 1e6f)) return 0;  // also NaN / negative / inf
+    if (!(v >= 9.9999e-5f && v < 1e6f)) return 0;  // also NaN / negative / inf
     const uint32_t bits = __float_as_uint(v);
     const int bexp = (int)((bits >> 23) & 0xFFu);
     const uint64_t m = bexp ? ((bits & 0x7FFFFFu) | 0x800000u) : (bits & 0x7FFFFFu);
     const int s = -((bexp ? bexp : 1) - 150);  // v = m * 2^-s, s in [4, 37] for the accepted range
-    const uint64_t P10[10] = {1ull, 10ull, 100ull, 1000ull, 10000ull, 100000ull, 1000000ull, 10000000ull, 100000000ull, 1000000000ull};
+    const uint64_t P10[11] = {1ull,         10ull,         100ull,         1000ull,         10000ull,      100000ull,
+                              1000000ull,   10000000ull,   100000000ull,   1000000000ull,   10000000000ull};
     int X = (int)floorf(log10f(v));  // decimal exponent, fixed below if the estimate is off by one
-    X = X < -4 ? -4 : (X > 5 ? 5 : X);
+    X = X < -5 ? -5 : (X > 5 ? 5 : X);
     uint64_t q = 0;
     for (int attempt = 0; attempt < 4; ++attempt) {
-        const int k = 5 - X;  // 0..9
-        const uint64_t N = m * P10[k];
-        q = N >> s;
-        const uint64_t r = N & ((1ull << s) - 1ull), half = 1ull << (s - 1);
-        if (r > half || (r == half && (q & 1ull))) ++q;
-        if (q < 100000ull) {
-            if (X == -4) return 0;  // below 1e-4 after all: exponent form
+        const int k = 5 - X;  // 0..10
+        const uint64_t N = m * P10[k];  // v 10^k = N 2^-s, below 2^58
+        const uint64_t t = N >> s;      // floor(v 10^k): v lies in decade X iff it has six digits (before rounding)
+        if (t < 100000ull) {
+            if (X == -5) return 0;
             --X;
             continue;
         }
-        if (q >= 1000000ull) {
-            if (q == 1000000ull && (N >> s) < 1000000ull) {  // the rounding carried into a seventh digit
-                q = 100000ull;
-                ++X;
-                if (X > 5) return 0;
-                break;
-            }
+        if (t >= 1000000ull) {
             if (X == 5) return 0;
             ++X;
             continue;
         }
+        const uint64_t r = N & ((1ull << s) - 1ull), half = 1ull << (s - 1);
+        q = t + ((r > half || (r == half && (t & 1ull))) ? 1ull : 0ull);
+        if (q == 1000000ull) {  // the rounding carried into a seventh digit: 10^(X+1)
+            q = 100000ull;
+            ++X;
+        }
         break;
     }
+    if (q == 0 || X < -4 || X > 5) return 0;  // exponent form (q == 0: the estimate was off by more than the loop fixes)
     char dg[6];
     for (int i = 5; i >= 0; --i) {
         dg[i] = (char)('0' + (int)(q % 10ull));
@@ -283,7 +283,7 @@ __global__ void __launch_bounds__(FIO_DEF_TPB) fio_deflate(const uint8_t* __rest
 // ---- deflate, one warp per block (the default).  A thread per block is bound by its own dependent chain (about
 // 2000 clocks a token: 0.7 s for a 5 M-record file); here the 32 lanes take 32 consecutive positions at a time:
 //   every lane hashes its four bytes and reads the candidate BEFORE any lane of the window inserts (so a match
-//   starts at least one window back), verifies and extends it on its own;
+//   starts at least one window back; of lanes with equal hashes the lowest inserts), verifies and extends it on its own;
 //   the token starts are then picked greedily from the left with one shuffle per token (uniform loop);
 //   the token bits (def_token, <= 31 each) go to their bit offsets (warp scan) in a 32-word ring in shared memory
 //   with atomicOr, and the words that became complete are stored to the block coalesced;
@@ -344,6 +344,16 @@ __global__ void __launch_bounds__(FIO_DEFW_WARPS * 32) fio_deflate_warp(const ui
         __syncwarp();
         if (can) head[h] = (uint16_t)pos;
         __syncwarp();
+        // lanes with equal hashes stored to one address, and CUDA does not say which of those stores lands: the lowest
+        // position is made to win (the lanes still above it store again until none is).  On the H100 it already has
+        // after the first store, so the loop only costs the check (the output is byte-identical to the unchecked store)
+        bool above = can && head[h] > pos;
+        while (__any_sync(FULL, above)) {
+            __syncwarp();
+            if (above) head[h] = (uint16_t)pos;
+            __syncwarp();
+            above = above && head[h] > pos;
+        }
         if (carry >= 32) {  // the whole window lies inside the last match
             carry -= 32;
             continue;
@@ -480,15 +490,11 @@ void fio_launch_splice_copy(const uint8_t* text, const int64_t* line_start, cons
     splice_copy<<<(unsigned)blocks, 256, 0, st>>>(text, line_start, recinfo, low, n, flags, out_start, score_txt, out, fallback);
 }
 cudaError_t fio_launch_deflate(const uint8_t* text, size_t n_bytes, const DefTables* tables, uint8_t* blocks, uint32_t* bsize,
-                               int n_blocks, cudaStream_t st) {
+                               int n_blocks, int encoder, cudaStream_t st) {
     if (n_blocks <= 0) return cudaSuccess;
-    static const bool thread_per_block = [] {  // UGVC_DEFLATE_THREADS=1: the thread-per-block encoder (A/B)
-        const char* e = getenv("UGVC_DEFLATE_THREADS");
-        return e && e[0] == '1';
-    }();
     cudaError_t e;
     // the attribute is set per call: it belongs to the current device, and lanes are driven from several host threads
-    if (!thread_per_block) {
+    if (encoder == FIO_ENC_WARP) {
         if ((e = cudaFuncSetAttribute(fio_deflate_warp, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FIO_DEFW_SMEM)) != cudaSuccess)
             return e;
         fio_deflate_warp<<<(n_blocks + FIO_DEFW_WARPS - 1) / FIO_DEFW_WARPS, FIO_DEFW_WARPS * 32, FIO_DEFW_SMEM, st>>>(
@@ -509,4 +515,22 @@ void fio_launch_pack(const uint8_t* blocks, const uint32_t* bsize, uint64_t* wid
 void fio_launch_widen(const uint32_t* bsize, uint64_t* wide, int n, cudaStream_t st) {
     if (n <= 0) return;
     fio_widen<<<(n + 255) / 256, 256, 0, st>>>(bsize, wide, n);
+}
+
+// test hook (ugvc_test_format_g): fio_format_g of every value into the 16-byte slot layout of splice_len (text in
+// bytes 0..14, zero padded; length in byte 15, 0 = left to the host writer)
+__global__ void __launch_bounds__(256) fio_test_format_g(const float* __restrict__ v, int64_t n, uint8_t* __restrict__ out) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        char num[16];
+        const int sl = fio_format_g(v[i], num);
+        uint8_t* st = out + (size_t)i * 16;
+        for (int c = 0; c < 15; ++c) st[c] = c < sl ? (uint8_t)num[c] : 0;
+        st[15] = (uint8_t)sl;
+    }
+}
+void fio_launch_test_format_g(const float* v, int64_t n, uint8_t* out, int sm_count, cudaStream_t st) {
+    if (n <= 0) return;
+    int64_t blocks = (n + 255) / 256;
+    if (blocks > (int64_t)sm_count * 16) blocks = (int64_t)sm_count * 16;
+    fio_test_format_g<<<(unsigned)blocks, 256, 0, st>>>(v, n, out);
 }

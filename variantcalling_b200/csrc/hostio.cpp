@@ -782,8 +782,8 @@ extern "C" int64_t ugvc_test_deflate_block_lanes(const uint8_t* in_, uint32_t n,
             w[lane] = can[lane] ? def_ld4(in + pos) : 0;
             cand[lane] = can[lane] ? head[DEFW_HASH(w[lane])] : 0xFFFFu;
         }
-        for (uint32_t lane = 0; lane < 32; ++lane)
-            if (can[lane]) head[DEFW_HASH(w[lane])] = (uint16_t)(p0 + lane);  // the highest lane wins, like the last store
+        for (uint32_t lane = 32; lane-- > 0;)  // of lanes with equal hashes the lowest wins, as in the kernel
+            if (can[lane]) head[DEFW_HASH(w[lane])] = (uint16_t)(p0 + lane);
         for (uint32_t lane = 0; lane < 32; ++lane) {
             const uint32_t pos = p0 + lane;
             len[lane] = dist[lane] = 0;

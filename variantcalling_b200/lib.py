@@ -112,6 +112,8 @@ SIGNATURES = {
     "ugvc_test_deflate_block_lanes": (C.c_int64, [_vp, C.c_uint32, _vp]),
     "ugvc_test_device_sigmoid": (C.c_int, [_vp, _vp, C.c_int, _vp, _vp]),
     "ugvc_test_k3_config": (C.c_int, [_vp, _vp]),
+    "ugvc_test_format_g": (C.c_int, [_vp, _vp, C.c_int64, _vp]),
+    "ugvc_test_device_deflate": (C.c_int, [_vp, _vp, _sz, C.c_int, _vp, _sz, _vp, _sz, C.POINTER(_sz), C.POINTER(_sz)]),
     "ugvc_bgzf_range_info": (C.c_int, [C.c_char_p, C.c_uint64, C.c_uint64, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64),
                                        C.POINTER(C.c_uint32), C.POINTER(C.c_uint64)]),
     "ugvc_filter_bgzf": (C.c_int, [_vp, C.c_int, _vp, _sz, C.c_uint32, C.c_uint64, C.c_double, C.c_int, _vp, _sz, C.POINTER(_sz),
@@ -428,6 +430,27 @@ class Context:
         kernel, tpb, nbuf, groups, nch, chunk, resident, grid, walk = (int(v) for v in out)
         return {"kernel": ("heap", "infer")[kernel], "tpb": tpb, "nbuf": nbuf, "groups": groups, "nch": nch, "chunk": chunk,
                 "resident": bool(resident), "grid": grid, "gs": tpb // groups, "walk": ("plain", "categorical")[walk]}
+
+    def test_format_g(self, values) -> np.ndarray:
+        """The record writer's "%g" on the device (test hook ugvc_test_format_g): an (n, 16) uint8 array, text in
+        bytes 0..14, its length in byte 15 (0 = left to the host writer)."""
+        v = np.ascontiguousarray(values, dtype=np.float32)
+        out = np.empty((v.size, 16), np.uint8)
+        if v.size:
+            self._check(self.lib.ugvc_test_format_g(self.h, _ptr(v), v.size, _ptr(out)))
+        return out
+
+    def test_device_deflate(self, data: bytes, encoder: int = 0) -> tuple[bytes, np.ndarray]:
+        """The file path's BGZF encoder on `data` (test hook ugvc_test_device_deflate; 0 = warp per block, 1 = thread
+        per block): (packed blocks, compressed size of each block).  Needs reserve() sized for the bytes."""
+        buf = np.frombuffer(data, dtype=np.uint8)
+        n_blocks = (buf.size + DEF_CHUNK - 1) // DEF_CHUNK
+        out = np.empty(n_blocks * 65536 + 1, np.uint8)
+        csize = np.empty(n_blocks + 1, np.uint32)
+        nb, nblk = C.c_size_t(), C.c_size_t()
+        self._check(self.lib.ugvc_test_device_deflate(self.h, _ptr(buf) if buf.size else None, buf.size, encoder, _ptr(out),
+                                                      out.size, _ptr(csize), csize.size, C.byref(nb), C.byref(nblk)))
+        return out[: nb.value].tobytes(), csize[: nblk.value].copy()
 
     def enable_stage_timing(self, on: bool = True):
         self._check(self.lib.ugvc_enable_stage_timing(self.h, int(on)))
