@@ -131,7 +131,9 @@ int ugvc_device_status_lane(ugvc_ctx* ctx, int lane, void* stream);
  * host memory whose uncompressed bytes are whole VCF data lines (<= the max_bytes of ugvc_reserve).
  * ugvc_submit_bgzf is ugvc_submit_batch for such input (results through ugvc_collect_batch as usual);
  * ugvc_bgzf_inflate_device only inflates into lane 0's text buffer and optionally copies the text
- * back (out_host may be NULL).  A corrupt block is UGVC_E_IO.  CRC32s are not verified on the device. */
+ * back (out_host may be NULL).  A block is refused (UGVC_E_IO, the message names the lowest such block) when its
+ * DEFLATE stream is one zlib refuses or does not end inside the payload, when it inflates to other than ISIZE bytes,
+ * or when their CRC32 differs from the footer's -- htslib's rule. */
 int ugvc_submit_bgzf(ugvc_ctx* ctx, int lane, const uint8_t* bgzf, size_t n_bytes, double threshold);
 int ugvc_bgzf_inflate_device(ugvc_ctx* ctx, const uint8_t* bgzf, size_t n_bytes, uint8_t* out_host, size_t capacity,
                              size_t* out_n);
@@ -392,6 +394,13 @@ int ugvc_test_format_g(ugvc_ctx* ctx, const float* v, int64_t n, uint8_t* out);
  * out_block_csize the size of each of the *out_n_blocks blocks of 57344 input bytes (none for n = 0). */
 int ugvc_test_device_deflate(ugvc_ctx* ctx, const uint8_t* data, size_t n, int encoder, uint8_t* out, size_t capacity,
                              uint32_t* out_block_csize, size_t block_capacity, size_t* out_bytes, size_t* out_n_blocks);
+/* Test hook: ugvc_bgzf_inflate_device (lane 0, same staging and kernels) with the decoder named: 0 = one warp per block
+ * (the default), 1 = one thread per block (UGVC_INFLATE_THREADS=1).  *out_n = the summed ISIZE; out receives the
+ * inflated bytes (a failed block's range is unspecified), block_rc the INF_* code (csrc/inflate.cuh; 0 = accepted,
+ * 9 = CRC32 mismatch) of each of the *out_n_blocks blocks with ISIZE > 0, in file order.  The host emulation has
+ * decoder 1 only (0 is UGVC_E_STATE there). */
+int ugvc_test_device_inflate(ugvc_ctx* ctx, const uint8_t* bgzf, size_t n_bytes, int decoder, uint8_t* out, size_t capacity,
+                             size_t* out_n, int32_t* block_rc, size_t block_capacity, size_t* out_n_blocks);
 /* Test hook: the K3 launch the loaded plan gets (also in the host emulation, which runs the same chunking).
  * out = {kernel (0 k3_heap, 1 k3_infer), threads per CTA, tile buffers per group, groups per CTA (records per tile:
  * threads / groups), trees one thread walks at once, forest chunk (k3_heap: trees, k3_infer: nodes; 0 for a linear

@@ -22,7 +22,8 @@ EMU_DIR = os.path.join(ROOT, "tests", "host_emu")
 EMU_LIB = os.path.join(EMU_DIR, "_build", "libugvc_emu.so")
 
 FILES = ["tests/test_gpu_parity.py", "tests/test_gpu_edges.py", "tests/test_gpu_fuzz.py", "tests/test_gpu_cnv.py",
-         "tests/test_gpu_cli.py", "tests/test_gpu_multiallelics.py", "tests/test_gpu_x_model_apply.py", "tests/test_gpu_x_deepvariant.py", "tests/test_gpu_x_bgzf.py", "tests/test_gpu_y_tiletok.py",
+         "tests/test_gpu_cli.py", "tests/test_gpu_multiallelics.py", "tests/test_gpu_x_model_apply.py", "tests/test_gpu_x_deepvariant.py", "tests/test_gpu_x_bgzf.py",
+         "tests/test_gpu_x_inflate_edges.py", "tests/test_gpu_y_tiletok.py",
          "tests/test_gpu_y_deviations.py", "tests/test_gpu_z_multiallelic_device.py", "tests/test_gpu_k3_shapes.py"]
 DEVICE_ONLY = ["tests/test_gpu_edges.py::test_device_generator_text_parity",  # the device synthetic generator
                "tests/test_gpu_parity.py::test_full_size_properties_batching_invariance",

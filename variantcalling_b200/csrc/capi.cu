@@ -210,6 +210,7 @@ extern "C" void ugvc_free(ugvc_ctx* ctx) {
 static size_t align8(size_t x) { return (x + 7) & ~(size_t)7; }
 
 static int find_host_tag(const ugvc_ctx* ctx, const std::string& name);
+static std::string inf_err_message(int word);
 
 // Tables of the tile kernel (k1_tok): every INFO key it may meet -- the plan's tags declared in ##INFO
 // plus the keys seen in the data (`info_keys`, "KEY;KEY!;..." as for the key order; '!' marks a key that
@@ -964,8 +965,7 @@ extern "C" int ugvc_collect_batch(ugvc_ctx* ctx, int lane, uint8_t* out_low_scor
     if (l.h_inf_err && *l.h_inf_err) {
         const int code = *l.h_inf_err;
         *l.h_inf_err = 0;
-        return fail(ctx, UGVC_E_IO, "BGZF inflate failed on the device (block " + std::to_string(code >> 8) + ", code " +
-                                        std::to_string(code & 0xFF) + ")");
+        return fail(ctx, UGVC_E_IO, inf_err_message(code));
     }
     const int rc = decode_error(ctx, *l.h_err);
     if (rc) return rc;
@@ -1048,13 +1048,25 @@ extern "C" int ugvc_device_status(ugvc_ctx* ctx, void* stream) {
 // ------------------------------------------------------------------------------------------
 // BGZF input: inflate on the device (inflate.cuh), then K0..K3 as usual
 // ------------------------------------------------------------------------------------------
+// The error word of an inflate launch: 0 when every block decoded, else the lowest failing block and its INF_* code
+// (atomicMax over the word keeps the lowest block: blocks are counted down from INF_ERR_BLOCKS).
+#define INF_ERR_BLOCKS 0x7FFFFF
+__host__ __device__ inline int inf_err_word(int b, int rc) { return ((INF_ERR_BLOCKS - b) << 8) | rc; }
+static std::string inf_err_message(int word) {
+    return "BGZF inflate failed on the device (block " + std::to_string(INF_ERR_BLOCKS - (word >> 8)) + ", code " +
+           std::to_string(word & 0xFF) + ")";
+}
+
+// block_rc: nullptr, or the INF_* code of every block (ugvc_test_device_inflate)
 __global__ void __launch_bounds__(64) bgzf_inflate_blocks(const uint8_t* __restrict__ comp, const uint64_t* __restrict__ blk,
                                                           size_t cap_blk, int n_blocks, uint8_t* __restrict__ out,
-                                                          int* __restrict__ err) {
+                                                          const DefTables* __restrict__ dt, int* __restrict__ err,
+                                                          int* __restrict__ block_rc) {
     for (int b = blockIdx.x * blockDim.x + threadIdx.x; b < n_blocks; b += gridDim.x * blockDim.x) {
         const int rc = inf_block(comp + blk[b], (uint32_t)blk[cap_blk + b], out + blk[2 * cap_blk + b],
-                                 (uint32_t)blk[3 * cap_blk + b]);
-        if (rc != INF_OK) atomicMax(err, (b << 8) | rc);
+                                 (uint32_t)blk[3 * cap_blk + b], *dt);
+        if (rc != INF_OK) atomicMax(err, inf_err_word(b, rc));
+        if (block_rc) block_rc[b] = rc;
     }
 }
 
@@ -1062,14 +1074,18 @@ __global__ void __launch_bounds__(64) bgzf_inflate_blocks(const uint8_t* __restr
 #define INFW_WARPS 16
 __global__ void __launch_bounds__(INFW_WARPS * 32) bgzf_inflate_warps(const uint8_t* __restrict__ comp, const uint64_t* __restrict__ blk,
                                                                       size_t cap_blk, int n_blocks, uint8_t* __restrict__ out,
-                                                                      int* __restrict__ err) {
+                                                                      const DefTables* __restrict__ dt, int* __restrict__ err,
+                                                                      int* __restrict__ block_rc) {
     extern __shared__ __align__(16) uint8_t infw_smem[];
     InfWarpTables& T = reinterpret_cast<InfWarpTables*>(infw_smem)[threadIdx.x >> 5];
     const int warp = (int)(blockIdx.x * INFW_WARPS + (threadIdx.x >> 5)), n_warps = (int)(gridDim.x * INFW_WARPS);
     for (int b = warp; b < n_blocks; b += n_warps) {
         const int rc = inf_block_warp(comp + blk[b], (uint32_t)blk[cap_blk + b], out + blk[2 * cap_blk + b],
-                                      (uint32_t)blk[3 * cap_blk + b], T);
-        if (rc != INF_OK && (threadIdx.x & 31) == 0) atomicMax(err, (b << 8) | rc);
+                                      (uint32_t)blk[3 * cap_blk + b], T, *dt);
+        if ((threadIdx.x & 31) == 0) {
+            if (rc != INF_OK) atomicMax(err, inf_err_word(b, rc));
+            if (block_rc) block_rc[b] = rc;
+        }
         __syncwarp();
     }
 }
@@ -1108,8 +1124,37 @@ static int scan_bgzf(ugvc_ctx* ctx, const uint8_t* p, size_t n, std::vector<uint
     return UGVC_OK;
 }
 
-// compressed bytes -> lane device buffers -> inflate into l.d_text; *n_text = uncompressed size
-static int stage_bgzf(ugvc_ctx* ctx, Lane& l, const uint8_t* bgzf, size_t n_bytes, size_t* n_text, size_t out_shift = 0) {
+// The CRC32 tables of the BGZF decoder and encoder (deflate.cuh), uploaded once per context
+static int def_tables(ugvc_ctx* ctx) {
+    static std::mutex tables_mu;  // lanes may take their first BGZF call on different host threads
+    std::lock_guard<std::mutex> lock(tables_mu);
+    if (!ctx->d_def_tables) {
+        DefTables* t = new DefTables();
+        def_build_tables(*t);
+        CU(cudaMalloc(&ctx->d_def_tables, sizeof(DefTables)));
+        const cudaError_t e = cudaMemcpy(ctx->d_def_tables, t, sizeof(DefTables), cudaMemcpyHostToDevice);
+        delete t;
+        CU(e);
+    }
+    return UGVC_OK;
+}
+
+enum { INF_DEC_WARP = 0, INF_DEC_THREAD = 1 };
+
+// UGVC_INFLATE_THREADS=1: the thread-per-block decoder instead of the warp-per-block one (A/B)
+static int inflate_decoder() {
+    static const int dec = [] {
+        const char* e = getenv("UGVC_INFLATE_THREADS");
+        return e && *e != '0' ? INF_DEC_THREAD : INF_DEC_WARP;
+    }();
+    return dec;
+}
+
+// compressed bytes -> lane device buffers -> inflate into l.d_text with `decoder` (INF_DEC_*); *n_text = uncompressed
+// size.  d_block_rc: nullptr, or room for the INF_* code of every block with ISIZE > 0.  The host emulation runs
+// inf_block whatever the decoder.
+static int stage_bgzf(ugvc_ctx* ctx, Lane& l, const uint8_t* bgzf, size_t n_bytes, int decoder, size_t* n_text,
+                      size_t out_shift = 0, int* d_block_rc = nullptr) {
     std::vector<uint64_t> coff, clen, uoff, ulen;
     size_t total = 0;
     int rc = scan_bgzf(ctx, bgzf, n_bytes, coff, clen, uoff, ulen, &total);
@@ -1117,6 +1162,9 @@ static int stage_bgzf(ugvc_ctx* ctx, Lane& l, const uint8_t* bgzf, size_t n_byte
     if (total + out_shift > ctx->cap_bytes) return fail(ctx, UGVC_E_ARG, "bgzf: the inflated batch is larger than the reserved max_bytes");
     for (auto& u : uoff) u += out_shift;
     const size_t nb = coff.size();
+    if (nb > INF_ERR_BLOCKS) return fail(ctx, UGVC_E_ARG, "bgzf: too many blocks in one call");
+    rc = def_tables(ctx);
+    if (rc) return rc;
     if (n_bytes + 8 > l.cap_comp) {
         cudaFree(l.d_comp);
         l.d_comp = nullptr;
@@ -1148,24 +1196,27 @@ static int stage_bgzf(ugvc_ctx* ctx, Lane& l, const uint8_t* bgzf, size_t n_byte
     CU(cudaMemcpyAsync(l.d_comp, bgzf, n_bytes, cudaMemcpyHostToDevice, st));
     CU(cudaMemcpyAsync(l.d_blk, l.h_blk.data(), 4 * l.cap_blk * sizeof(uint64_t), cudaMemcpyHostToDevice, st));
 #ifdef UGVC_HOST_EMU
+    (void)decoder;
     for (size_t i = 0; i < nb; ++i) {
-        const int e = inf_block(l.d_comp + coff[i], (uint32_t)clen[i], l.d_text + uoff[i], (uint32_t)ulen[i]);
-        if (e != INF_OK && *l.d_inf_err < (int)((i << 8) | e)) *l.d_inf_err = (int)((i << 8) | e);
+        const int e = inf_block(l.d_comp + coff[i], (uint32_t)clen[i], l.d_text + uoff[i], (uint32_t)ulen[i], *ctx->d_def_tables);
+        if (e != INF_OK && *l.d_inf_err < inf_err_word((int)i, e)) *l.d_inf_err = inf_err_word((int)i, e);
+        if (d_block_rc) d_block_rc[i] = e;
     }
 #else
-    static const bool per_thread = getenv("UGVC_INFLATE_THREADS") && *getenv("UGVC_INFLATE_THREADS") != '0';  // A/B: one thread per block
-    if (per_thread) {
+    if (decoder == INF_DEC_THREAD) {
         const int threads = 64;
         int grid = (int)((nb + threads - 1) / threads);
         if (grid > ctx->sm_count * 16) grid = ctx->sm_count * 16;
-        bgzf_inflate_blocks<<<grid, threads, 0, st>>>(l.d_comp, l.d_blk, l.cap_blk, (int)nb, l.d_text, l.d_inf_err);
+        bgzf_inflate_blocks<<<grid, threads, 0, st>>>(l.d_comp, l.d_blk, l.cap_blk, (int)nb, l.d_text, ctx->d_def_tables,
+                                                      l.d_inf_err, d_block_rc);
     } else {  // one warp per block, tables in shared memory
         const size_t smem = INFW_WARPS * sizeof(InfWarpTables);
         // per call: a function attribute belongs to the current device, and lanes are driven from several host threads
         CU(cudaFuncSetAttribute(bgzf_inflate_warps, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         int grid = (int)((nb + INFW_WARPS - 1) / INFW_WARPS);
         if (grid > ctx->sm_count * 3) grid = ctx->sm_count * 3;
-        bgzf_inflate_warps<<<grid, INFW_WARPS * 32, smem, st>>>(l.d_comp, l.d_blk, l.cap_blk, (int)nb, l.d_text, l.d_inf_err);
+        bgzf_inflate_warps<<<grid, INFW_WARPS * 32, smem, st>>>(l.d_comp, l.d_blk, l.cap_blk, (int)nb, l.d_text,
+                                                                 ctx->d_def_tables, l.d_inf_err, d_block_rc);
     }
     CU(cudaGetLastError());
 #endif
@@ -1183,7 +1234,7 @@ extern "C" int ugvc_submit_bgzf(ugvc_ctx* ctx, int lane, const uint8_t* bgzf, si
     Lane& l = ctx->lanes[lane];
     if (l.submitted) return fail(ctx, UGVC_E_STATE, "submit_bgzf: lane already has a batch in flight");
     size_t n_text = 0;
-    int rc = stage_bgzf(ctx, l, bgzf, n_bytes, &n_text);
+    int rc = stage_bgzf(ctx, l, bgzf, n_bytes, inflate_decoder(), &n_text);
     if (rc) return rc;
     CU(cudaMemsetAsync(l.d_text + n_text, '\n', TEXT_SLACK, l.stream));
     rc = enqueue_kernels(ctx, l, l.d_text, n_text, threshold, l.b.low_score, l.b.probs, l.b.qual, l.b.recinfo,
@@ -1205,20 +1256,56 @@ extern "C" int ugvc_bgzf_inflate_device(ugvc_ctx* ctx, const uint8_t* bgzf, size
     Lane& l = ctx->lanes[0];
     if (l.submitted) return fail(ctx, UGVC_E_STATE, "bgzf_inflate_device: lane 0 has a batch in flight");
     size_t n_text = 0;
-    int rc = stage_bgzf(ctx, l, bgzf, n_bytes, &n_text);
+    int rc = stage_bgzf(ctx, l, bgzf, n_bytes, inflate_decoder(), &n_text);
     if (rc) return rc;
     if (out_n) *out_n = n_text;
     CU(cudaStreamSynchronize(l.stream));
     if (l.h_inf_err && *l.h_inf_err) {
         const int code = *l.h_inf_err;
         *l.h_inf_err = 0;
-        return fail(ctx, UGVC_E_IO, "BGZF inflate failed on the device (block " + std::to_string(code >> 8) + ", code " +
-                                        std::to_string(code & 0xFF) + ")");
+        return fail(ctx, UGVC_E_IO, inf_err_message(code));
     }
     if (out_host) {
         if (n_text > capacity) return fail(ctx, UGVC_E_ARG, "bgzf_inflate_device: output capacity too small");
         CU(cudaMemcpy(out_host, l.d_text, n_text, cudaMemcpyDeviceToHost));
     }
+    return UGVC_OK;
+}
+
+extern "C" int ugvc_test_device_inflate(ugvc_ctx* ctx, const uint8_t* bgzf, size_t n_bytes, int decoder, uint8_t* out,
+                                        size_t capacity, size_t* out_n, int32_t* block_rc, size_t block_capacity,
+                                        size_t* out_n_blocks) {
+    // test hook: ugvc_bgzf_inflate_device with the decoder named, reporting the INF_* code of every block instead of
+    // the lowest failing one
+    if (!ctx || (n_bytes && !bgzf) || !out_n || !out_n_blocks || (decoder != INF_DEC_WARP && decoder != INF_DEC_THREAD))
+        return UGVC_E_ARG;
+#ifdef UGVC_HOST_EMU
+    if (decoder == INF_DEC_WARP) return fail(ctx, UGVC_E_STATE, "the warp-per-block decoder is not part of the host emulation");
+#endif
+    if (ctx->lanes.empty()) return fail(ctx, UGVC_E_STATE, "test_device_inflate: reserve first (the text lands in lane 0)");
+    CU(cudaSetDevice(ctx->device));
+    Lane& l = ctx->lanes[0];
+    if (l.submitted) return fail(ctx, UGVC_E_STATE, "test_device_inflate: lane 0 has a batch in flight");
+    std::vector<uint64_t> coff, clen, uoff, ulen;
+    size_t n_text = 0;
+    int rc = scan_bgzf(ctx, bgzf, n_bytes, coff, clen, uoff, ulen, &n_text);
+    if (rc) return rc;
+    const size_t nb = coff.size();
+    if (nb > block_capacity || (nb && !block_rc)) return fail(ctx, UGVC_E_ARG, "test_device_inflate: more blocks than block_capacity");
+    if (n_text > capacity || (n_text && !out)) return fail(ctx, UGVC_E_ARG, "test_device_inflate: output capacity too small");
+    struct DevFree {
+        int* p = nullptr;
+        ~DevFree() { cudaFree(p); }
+    } d_rc;
+    CU(cudaMalloc(&d_rc.p, (nb ? nb : 1) * sizeof(int)));
+    rc = stage_bgzf(ctx, l, bgzf, n_bytes, decoder, &n_text, 0, d_rc.p);
+    if (rc) return rc;
+    CU(cudaStreamSynchronize(l.stream));
+    if (l.h_inf_err) *l.h_inf_err = 0;  // reported through block_rc
+    if (nb) CU(cudaMemcpy(block_rc, d_rc.p, nb * sizeof(int), cudaMemcpyDeviceToHost));
+    if (n_text) CU(cudaMemcpy(out, l.d_text, n_text, cudaMemcpyDeviceToHost));
+    *out_n = n_text;
+    *out_n_blocks = nb;
     return UGVC_OK;
 }
 
@@ -1262,16 +1349,7 @@ static int file_bufs(ugvc_ctx* ctx, Lane& l) {
     CU(cudaHostAlloc(&f.h_fallback, sizeof(int), cudaHostAllocDefault));
     CU(cudaHostAlloc(&f.h_total, sizeof(int64_t), cudaHostAllocDefault));
     for (auto& e : f.ev) CU(cudaEventCreate(&e));
-    static std::mutex tables_mu;  // lanes may take their first file-path call on different host threads
-    std::lock_guard<std::mutex> lock(tables_mu);
-    if (!ctx->d_def_tables) {
-        DefTables* t = new DefTables();
-        def_build_tables(*t);
-        CU(cudaMalloc(&ctx->d_def_tables, sizeof(DefTables)));
-        CU(cudaMemcpy(ctx->d_def_tables, t, sizeof(DefTables), cudaMemcpyHostToDevice));
-        delete t;
-    }
-    return UGVC_OK;
+    return def_tables(ctx);
 }
 
 // UGVC_DEFLATE_THREADS=1: the thread-per-block encoder instead of the warp-per-block one (A/B)
@@ -1320,7 +1398,7 @@ extern "C" int ugvc_filter_bgzf(ugvc_ctx* ctx, int lane, const uint8_t* bgzf, si
     // ---- compressed blocks -> text on the device, the range's first byte 16-byte aligned
     const size_t shift = (16 - (skip_head & 15u)) & 15u;
     size_t total = 0;
-    rc = stage_bgzf(ctx, l, bgzf, n_bytes, &total, shift);
+    rc = stage_bgzf(ctx, l, bgzf, n_bytes, inflate_decoder(), &total, shift);
     if (rc) return rc;
     if (skip_head > total) return fail(ctx, UGVC_E_ARG, "filter_bgzf: skip_head beyond the inflated blocks");
     const size_t n_text = take_bytes ? (size_t)take_bytes : total - skip_head;
@@ -1338,8 +1416,7 @@ extern "C" int ugvc_filter_bgzf(ugvc_ctx* ctx, int lane, const uint8_t* bgzf, si
     if (l.h_inf_err && *l.h_inf_err) {
         const int code = *l.h_inf_err;
         *l.h_inf_err = 0;
-        return fail(ctx, UGVC_E_IO, "BGZF inflate failed on the device (block " + std::to_string(code >> 8) + ", code " +
-                                        std::to_string(code & 0xFF) + ")");
+        return fail(ctx, UGVC_E_IO, inf_err_message(code));
     }
     rc = decode_error(ctx, *l.h_err);
     if (rc) return rc;

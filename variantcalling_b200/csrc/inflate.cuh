@@ -4,18 +4,20 @@
 // (filter_variants_pipeline.py:106,115); moving the decode to the GPU lets the host ship the
 // *compressed* bytes over PCIe (4-5x fewer for VCF text), the link that bounds the end-to-end rate.
 //
-// One thread per BGZF block (<= 64 KiB in, <= 65280 B out, self-contained: no history crosses
-// blocks).  Each thread keeps a 64-bit bit buffer, decodes stored / fixed / dynamic blocks with a
-// 9-bit look-up table for the literal-length code and a 7-bit one for the distance code (longer
-// codes fall back to a canonical bit-by-bit walk), and writes its output range directly.  The tables
-// live in the thread's local memory (about 3.9 KB with the code-length scratch).  The bit buffer is
-// refilled with aligned 32-bit loads; long matches far enough behind are moved as aligned 8-byte words
-// (the source realigned with a funnel shift), shorter ones in groups of eight independent byte loads.
-// Written for exactness first (byte-identical with zlib on every block type, checked on the host
-// emulation; first GPU timing pending): literal stores are still byte-wide, and a warp-cooperative
-// decoder (one block per warp, tables in shared memory) is the next step if the profile asks for it.
+// Every BGZF block is self-contained (<= 64 KiB in, <= 64 KiB out, no history crosses blocks), so blocks are
+// decoded independently.  Two decoders share the Huffman code builder and the symbol decoder below:
+//  - inf_block_warp (the default, `bgzf_inflate_warps`): one warp per block.  The bit stream is decoded
+//    warp-uniformly on tables in shared memory (10-bit literal-length and 8-bit distance look-up tables), the byte
+//    moves of matches and stored blocks are spread over the lanes.
+//  - inf_block (`bgzf_inflate_blocks`, UGVC_INFLATE_THREADS=1, and the host emulation): one thread per block with
+//    9-bit / 7-bit tables in local memory, long matches moved as aligned 8-byte words.
+// Codes longer than a table fall back to a canonical bit-by-bit walk.  Both decoders accept exactly what zlib's
+// inflate accepts for a raw stream that ends inside the payload, and then check the block the way htslib's reader
+// does: the output length must equal ISIZE and its CRC32 (def_crc_slice, deflate.cuh) the gzip footer's.
 #pragma once
 #include <stdint.h>
+
+#include "deflate.cuh"
 
 #ifndef __CUDACC__
 #ifndef __host__
@@ -34,7 +36,14 @@ enum : int {
     INF_OUTPUT_OVERRUN = 6,
     INF_INPUT_OVERRUN = 7,
     INF_SIZE_MISMATCH = 8,
+    INF_BAD_CRC = 9,
 };
+
+// the CRC32 of the gzip footer, which follows the DEFLATE payload in[0, n_in)
+__host__ __device__ inline uint32_t inf_footer_crc(const uint8_t* in, uint32_t n_in) {
+    const uint8_t* f = in + n_in;
+    return (uint32_t)f[0] | ((uint32_t)f[1] << 8) | ((uint32_t)f[2] << 16) | ((uint32_t)f[3] << 24);
+}
 
 #define INF_LIT_BITS 9
 #define INF_DIST_BITS 7
@@ -77,7 +86,10 @@ struct InfBits {
 
 // Canonical Huffman code of `n` symbols with lengths len[0..n): count[], first-symbol offsets and the
 // sorted symbol list for the slow path, plus a `bits`-wide look-up table: entry = (symbol << 4) | length,
-// 0 for prefixes of longer codes.  Returns false for an over-subscribed set of lengths.
+// 0 for prefixes of longer codes.  Returns false for a set of lengths zlib's inflate_table refuses: an
+// over-subscribed one, or an incomplete one -- except that a literal-length or distance code may consist of a
+// single code of length 1, and a distance code may have no codes at all (a literal-only block).  The code-length
+// code (`code_lengths`) must be complete.
 struct InfCode {
     uint16_t count[INF_MAX_BITS + 1];
     uint16_t symbol[288];
@@ -92,17 +104,19 @@ __host__ __device__ inline uint32_t inf_reverse(uint32_t code, int len) {
     return r;
 }
 
-__host__ __device__ inline bool inf_build(InfCode& c, const uint8_t* len, int n, uint16_t* lut, int bits) {
+__host__ __device__ inline bool inf_build(InfCode& c, const uint8_t* len, int n, uint16_t* lut, int bits,
+                                          bool code_lengths = false) {
     for (int i = 0; i <= INF_MAX_BITS; ++i) c.count[i] = 0;
     for (int i = 0; i < n; ++i) c.count[len[i]]++;
     for (int i = 0; i < (1 << bits); ++i) lut[i] = 0;
-    if (c.count[0] == n) return true;  // no codes at all: legal for the distance code of a literal-only block
+    if (c.count[0] == n) return !code_lengths;  // no codes at all: legal for the distance code of a literal-only block
     int left = 1;
     for (int l = 1; l <= INF_MAX_BITS; ++l) {
         left <<= 1;
         left -= c.count[l];
         if (left < 0) return false;  // over-subscribed
     }
+    if (left > 0 && (code_lengths || c.count[0] != n - 1 || c.count[1] != 1)) return false;  // incomplete
     uint16_t offs[INF_MAX_BITS + 2];
     offs[1] = 0;
     for (int l = 1; l < INF_MAX_BITS; ++l) offs[l + 1] = offs[l] + c.count[l];
@@ -149,8 +163,9 @@ __host__ __device__ inline int inf_decode(InfBits& b, const InfCode& c, const ui
     return -1;
 }
 
-// Inflate one raw DEFLATE stream of n_in bytes into exactly n_out bytes.  Returns INF_*.
-__host__ __device__ inline int inf_block(const uint8_t* in, uint32_t n_in, uint8_t* out, uint32_t n_out) {
+// Inflate one raw DEFLATE stream of n_in bytes into exactly n_out bytes whose CRC32 is the one in the gzip footer at
+// in + n_in.  Returns INF_*.
+__host__ __device__ inline int inf_block(const uint8_t* in, uint32_t n_in, uint8_t* out, uint32_t n_out, const DefTables& T) {
     const uint16_t LEN_BASE[29] = {3, 4, 5, 6, 7, 8, 9, 10, 11, 13, 15, 17, 19, 23, 27, 31, 35, 43, 51, 59, 67, 83, 99, 115, 131, 163, 195, 227, 258};
     const uint8_t LEN_EXTRA[29] = {0, 0, 0, 0, 0, 0, 0, 0, 1, 1, 1, 1, 2, 2, 2, 2, 3, 3, 3, 3, 4, 4, 4, 4, 5, 5, 5, 5, 0};
     const uint16_t DIST_BASE[30] = {1, 2, 3, 4, 5, 7, 9, 13, 17, 25, 33, 49, 65, 97, 129, 193, 257, 385, 513, 769, 1025, 1537, 2049, 3073, 4097, 6145, 8193, 12289, 16385, 24577};
@@ -190,8 +205,8 @@ __host__ __device__ inline int inf_block(const uint8_t* in, uint32_t n_in, uint8
                 for (int i = 256; i < 280; ++i) lens[i] = 7;
                 for (int i = 280; i < 288; ++i) lens[i] = 8;
                 inf_build(lit, lens, 288, lit_lut, INF_LIT_BITS);
-                for (int i = 0; i < 30; ++i) lens[i] = 5;
-                inf_build(dist, lens, 30, dist_lut, INF_DIST_BITS);
+                for (int i = 0; i < 32; ++i) lens[i] = 5;  // complete: distance codes 30 and 31 decode and are refused
+                inf_build(dist, lens, 32, dist_lut, INF_DIST_BITS);
             } else {  // dynamic code
                 const int hlit = (int)b.take(5) + 257, hdist = (int)b.take(5) + 1, hclen = (int)b.take(4) + 4;
                 if (hlit > 286 || hdist > 30) return INF_BAD_CODE_LENGTHS;
@@ -204,7 +219,7 @@ __host__ __device__ inline int inf_block(const uint8_t* in, uint32_t n_in, uint8
                 }
                 InfCode clc;
                 uint16_t cl_lut[1 << 7];
-                if (!inf_build(clc, cl, 19, cl_lut, 7)) return INF_BAD_CODE_LENGTHS;
+                if (!inf_build(clc, cl, 19, cl_lut, 7, true)) return INF_BAD_CODE_LENGTHS;
                 int i = 0;
                 while (i < hlit + hdist) {
                     b.refill();
@@ -290,7 +305,8 @@ __host__ __device__ inline int inf_block(const uint8_t* in, uint32_t n_in, uint8
         if (last) break;
     }
     if (b.pos - (uint32_t)(b.cnt >> 3) > n_in) return INF_INPUT_OVERRUN;
-    return op == n_out ? INF_OK : INF_SIZE_MISMATCH;
+    if (op != n_out) return INF_SIZE_MISMATCH;
+    return def_crc_slice(T, out, n_out) == inf_footer_crc(in, n_in) ? INF_OK : INF_BAD_CRC;
 }
 
 #if defined(__CUDACC__) && !defined(UGVC_HOST_EMU)
@@ -320,7 +336,7 @@ __constant__ uint8_t INFW_DIST_EXTRA[30] = {0, 0, 0, 0, 1, 1, 2, 2, 3, 3, 4, 4, 
 __constant__ uint8_t INFW_CL_ORDER[19] = {16, 17, 18, 0, 8, 7, 9, 6, 10, 5, 11, 4, 12, 3, 13, 2, 14, 1, 15};
 
 __device__ __forceinline__ int inf_block_warp(const uint8_t* __restrict__ in, uint32_t n_in, uint8_t* out, uint32_t n_out,
-                                              InfWarpTables& T) {
+                                              InfWarpTables& T, const DefTables& D) {
     const unsigned lane = threadIdx.x & 31u;
     const volatile uint8_t* vout = out;
     InfBits b;
@@ -356,8 +372,8 @@ __device__ __forceinline__ int inf_block_warp(const uint8_t* __restrict__ in, ui
                     for (int i = 256; i < 280; ++i) T.lens[i] = 7;
                     for (int i = 280; i < 288; ++i) T.lens[i] = 8;
                     inf_build(T.lit, T.lens, 288, T.lit_lut, INFW_LIT_BITS);
-                    for (int i = 0; i < 30; ++i) T.lens[i] = 5;
-                    inf_build(T.dist, T.lens, 30, T.dist_lut, INFW_DIST_BITS);
+                    for (int i = 0; i < 32; ++i) T.lens[i] = 5;  // complete: distance codes 30 and 31 decode and are refused
+                    inf_build(T.dist, T.lens, 32, T.dist_lut, INFW_DIST_BITS);
                 }
             } else {  // dynamic code: the header is decoded by every lane (uniform), the tables are built by lane 0
                 const int hlit = (int)b.take(5) + 257, hdist = (int)b.take(5) + 1, hclen = (int)b.take(4) + 4;
@@ -374,7 +390,7 @@ __device__ __forceinline__ int inf_block_warp(const uint8_t* __restrict__ in, ui
                     for (int i = 0; i < 19; ++i) cl[i] = 0;
                     for (int i = 0; i < hclen; ++i) cl[INFW_CL_ORDER[i]] = (uint8_t)cl3[i];
                     // the code-length code shares the distance tables' storage until they are built
-                    if (!inf_build(T.dist, cl, 19, T.dist_lut, 7)) err = INF_BAD_CODE_LENGTHS;
+                    if (!inf_build(T.dist, cl, 19, T.dist_lut, 7, true)) err = INF_BAD_CODE_LENGTHS;
                 }
                 __syncwarp();
                 err = __shfl_sync(0xffffffffu, err, 0);
@@ -448,6 +464,20 @@ __device__ __forceinline__ int inf_block_warp(const uint8_t* __restrict__ in, ui
         if (last) break;
     }
     if (b.pos - (uint32_t)(b.cnt >> 3) > n_in) return INF_INPUT_OVERRUN;
-    return op == n_out ? INF_OK : INF_SIZE_MISMATCH;
+    if (op != n_out) return INF_SIZE_MISMATCH;
+    // CRC32: every lane one contiguous slice, the slices' CRCs combined pairwise up the warp
+    __syncwarp();  // every lane's stores are visible
+    const uint32_t per = (n_out + 31u) / 32u, lo = lane * per < n_out ? lane * per : n_out;
+    uint32_t len = n_out - lo < per ? n_out - lo : per;
+    uint32_t crc = def_crc_slice(D, out + lo, len);
+    for (unsigned s = 1; s < 32u; s <<= 1) {
+        const uint32_t crc_b = __shfl_down_sync(0xffffffffu, crc, s), len_b = __shfl_down_sync(0xffffffffu, len, s);
+        if ((lane & (2u * s - 1u)) == 0) {
+            crc = def_crc_combine(D, crc, crc_b, len_b);
+            len += len_b;
+        }
+    }
+    crc = __shfl_sync(0xffffffffu, crc, 0);
+    return crc == inf_footer_crc(in, n_in) ? INF_OK : INF_BAD_CRC;
 }
 #endif

@@ -114,6 +114,7 @@ SIGNATURES = {
     "ugvc_test_k3_config": (C.c_int, [_vp, _vp]),
     "ugvc_test_format_g": (C.c_int, [_vp, _vp, C.c_int64, _vp]),
     "ugvc_test_device_deflate": (C.c_int, [_vp, _vp, _sz, C.c_int, _vp, _sz, _vp, _sz, C.POINTER(_sz), C.POINTER(_sz)]),
+    "ugvc_test_device_inflate": (C.c_int, [_vp, _vp, _sz, C.c_int, _vp, _sz, C.POINTER(_sz), _vp, _sz, C.POINTER(_sz)]),
     "ugvc_bgzf_range_info": (C.c_int, [C.c_char_p, C.c_uint64, C.c_uint64, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64),
                                        C.POINTER(C.c_uint32), C.POINTER(C.c_uint64)]),
     "ugvc_filter_bgzf": (C.c_int, [_vp, C.c_int, _vp, _sz, C.c_uint32, C.c_uint64, C.c_double, C.c_int, _vp, _sz, C.POINTER(_sz),
@@ -451,6 +452,18 @@ class Context:
         self._check(self.lib.ugvc_test_device_deflate(self.h, _ptr(buf) if buf.size else None, buf.size, encoder, _ptr(out),
                                                       out.size, _ptr(csize), csize.size, C.byref(nb), C.byref(nblk)))
         return out[: nb.value].tobytes(), csize[: nblk.value].copy()
+
+    def test_device_inflate(self, bgzf: bytes, decoder: int = 0) -> tuple[np.ndarray, np.ndarray]:
+        """The device BGZF decoder on whole BGZF blocks (test hook ugvc_test_device_inflate; 0 = warp per block, 1 =
+        thread per block): (inflated bytes, INF_* code of each block with ISIZE > 0).  Needs reserve() sized for the
+        output; a failed block's bytes are unspecified."""
+        buf = np.frombuffer(bgzf, dtype=np.uint8)
+        out = np.empty(max(1, self.cap_bytes), np.uint8)
+        rc = np.empty(max(1, buf.size // 26 + 1), np.int32)  # a BGZF block is at least 26 bytes
+        n, nblk = C.c_size_t(), C.c_size_t()
+        self._check(self.lib.ugvc_test_device_inflate(self.h, _ptr(buf) if buf.size else None, buf.size, decoder, _ptr(out),
+                                                      out.size, C.byref(n), _ptr(rc), rc.size, C.byref(nblk)))
+        return out[: n.value], rc[: nblk.value].copy()
 
     def enable_stage_timing(self, on: bool = True):
         self._check(self.lib.ugvc_enable_stage_timing(self.h, int(on)))
