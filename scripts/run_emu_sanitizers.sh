@@ -10,6 +10,7 @@ export UGVC_LIB_PATH="$PWD/tests/host_emu/_build_san/libugvc_emu.so"
 python -m pytest -q -m gpu -p no:cacheprovider tests/test_gpu_parity.py tests/test_gpu_edges.py tests/test_gpu_fuzz.py \
     tests/test_gpu_cnv.py tests/test_gpu_cli.py tests/test_gpu_multiallelics.py tests/test_gpu_x_model_apply.py \
     tests/test_gpu_x_deepvariant.py tests/test_gpu_x_bgzf.py tests/test_gpu_x_inflate_edges.py tests/test_gpu_y_tiletok.py tests/test_gpu_y_deviations.py \
+    tests/test_gpu_feature_edges.py \
     tests/test_gpu_z_multiallelic_device.py \
     --deselect tests/test_gpu_edges.py::test_device_generator_text_parity \
     --deselect tests/test_gpu_parity.py::test_full_size_properties_batching_invariance 2>&1 | tee /tmp/emu_san_tests.log | tail -2

@@ -8,6 +8,14 @@ reference does or asserts the stated difference, so that none of them can drift 
  2. integer tag values beyond 2^24 with a logistic-regression model: sklearn evaluates the frame in fp64, the
     feature matrix on the device is fp32 (X.astype(float32), what the tree models see in the reference too): the
     probability may differ, by no more than the coefficient times the fp32 rounding of the value.
+ 3. an Integer literal outside int32: htslib refuses it, the oracle reader (Python int) keeps it; the device refuses
+    the record (UgvcDataError naming it).
+ 4. an empty numeric value ("SOR=", "LONG_HMER="): the reference reads None and imputes it; the device refuses the
+    record as a bad literal.
+ 5. an empty string value where the reference indexes or iterates it ("X_HIN=" is (), "X_LM=" under Number=1 is None):
+    the reference raises, the device scores a string without a base (0).
+The cases of 3-5 are in tests/feature_cases.py (``deviation``); the reference side is pinned by
+tests/test_feature_cases_cpu.py.
 """
 import numpy as np
 import pandas as pd
@@ -93,3 +101,32 @@ def test_large_integers_under_logistic_regression(gpu_ctx, base):
     np.testing.assert_allclose(res["probs"][others], exp["probs"][others], atol=1e-6, rtol=0)
     margin_err = abs(float(model.coef_[0][col])) * abs(float(np.float32(big)) - big)
     assert abs(float(res["probs"][5, 1]) - float(exp["probs"][5, 1])) <= margin_err * 0.25 + 1e-6  # d sigmoid <= 1/4
+
+
+@pytest.mark.parametrize("name", ["ss", "ss1", "dvx", "cnv"])
+def test_corpus_deviations(gpu_ctx, name):
+    from tests import feature_cases as FC
+    from tests.test_gpu_feature_edges import fitted, plan_of, run
+
+    fl, tr, _ = fitted(name)
+    plan = plan_of(name, "gb8")
+    clean = fl["lines"][:40]
+    learn = ("\n".join(fl["lines"][:120]) + "\n").encode()
+    cases = [c for c in FC.cases_of(name) if c.deviation]
+    assert cases
+    for c in cases:
+        line = FC.apply(FC.base_record(fl), c.edits)
+        if c.want == FC.RAISES:
+            with pytest.raises((ValueError, KeyError, AssertionError, TypeError, IndexError)):
+                FC.reference_matrix(fl, clean + [line], tr)
+        else:
+            FC.reference_matrix(fl, clean + [line], tr)
+        for legacy in (False, True):
+            res = run(gpu_ctx, plan.blob, clean + [line], learn, legacy)
+            if c.on_device == FC.RAISES:
+                assert res.get("error", (None,))[0] == len(clean), (c.name, legacy)
+                continue
+            assert "error" not in res, (c.name, legacy, res.get("error"))
+            for feat, v in c.on_device.items():
+                got = res["feats"][len(clean), plan.feature_names.index(feat)]
+                assert got.tobytes() == np.float32(v).tobytes(), (c.name, feat, got)

@@ -551,7 +551,10 @@ __device__ __noinline__ Cur parse_value(RawOut o, int t, unsigned kind, Cur c, u
         return r.c;
     }
     if (whole == RED_STRNUM) {
-        const NumCur r = parse_num_cur(c);
+        // pd.to_numeric ignores spaces around the number (the tile kernel hands such values over to this parser)
+        while (c.peek() == ' ') c.adv();
+        NumCur r = parse_num_cur(c);
+        while (r.st == NUM_OK && r.c.peek() == ' ') r.c.adv();
         const unsigned ch = r.c.peek();
         const bool ok = r.st == NUM_OK && (ch == vend || ch == '\t' || ch == '\n') && !isnan(r.v);
         store_slot(o, tg.whole_slot, ok ? __float_as_uint((float)r.v) : RAW_ERR);
@@ -883,6 +886,18 @@ __device__ __forceinline__ float k2_apply(uint32_t bits, const PlanFeature& pf, 
     return v;
 }
 
+__device__ __forceinline__ void k2_combine_one(const PlanCombine cb, uint32_t bbits, float& a, long long rec, bool live,
+                                               unsigned long long* err) {
+    const bool b_null = bbits == RAW_ABSENT || bbits == RAW_MISSING;
+    if (bbits == RAW_ERR && live) atomicMin(err, ugvc_pack_error(rec, cb.feature, REASON_BAD_VALUE));
+    const float bv = __uint_as_float(bbits);
+    const float r = isnan(a) ? (b_null ? a : bv) : (b_null ? a : fmaxf(a, bv));
+    if (isnan(r) && live) atomicMin(err, ugvc_pack_error(rec, cb.feature, REASON_NULL_FEATURE));
+    // an infinite operand wins the max: the model's input check raises "Input X contains infinity"
+    if (isinf(r) && live) atomicMin(err, ugvc_pack_error(rec, cb.feature, REASON_BAD_VALUE));
+    a = r;
+}
+
 __global__ void __launch_bounds__(K2_TPB) k2_features(const __grid_constant__ DevPlan plan,
                                                       const uint32_t* __restrict__ raw, size_t row_stride,
                                                       const int64_t* __restrict__ n_records_p,
@@ -919,12 +934,7 @@ __global__ void __launch_bounds__(K2_TPB) k2_features(const __grid_constant__ De
             float* av = &a.x;
 #pragma unroll
             for (int i = 0; i < 4; ++i) {
-                const bool b_null = bb[i] == RAW_ABSENT || bb[i] == RAW_MISSING;
-                if (bb[i] == RAW_ERR && i < live) atomicMin(err, ugvc_pack_error(rec + i, cb.feature, REASON_BAD_VALUE));
-                const float bv = __uint_as_float(bb[i]);
-                const float r = isnan(av[i]) ? (b_null ? av[i] : bv) : (b_null ? av[i] : fmaxf(av[i], bv));
-                if (isnan(r) && i < live) atomicMin(err, ugvc_pack_error(rec + i, cb.feature, REASON_NULL_FEATURE));
-                av[i] = r;
+                k2_combine_one(cb, bb[i], av[i], rec + i, i < live, err);
             }
             *dst = a;
         }
@@ -1311,15 +1321,6 @@ k3_infer(const __grid_constant__ DevPlan plan, const float* __restrict__ feats, 
 // addresses broadcast), so a level costs three conflict-free wavefronts (feature byte, threshold, x).  The
 // feature tile is assembled straight from K1's raw slots with the fitted transformer's missing / absent
 // policies (what k2_features did in a pass of its own), or copied from a dense matrix (ugvc_predict_features).
-__device__ __forceinline__ void k2_combine_one(const PlanCombine cb, uint32_t bbits, float& a, long long rec, bool live,
-                                               unsigned long long* err) {
-    const bool b_null = bbits == RAW_ABSENT || bbits == RAW_MISSING;
-    if (bbits == RAW_ERR && live) atomicMin(err, ugvc_pack_error(rec, cb.feature, REASON_BAD_VALUE));
-    const float bv = __uint_as_float(bbits);
-    const float r = isnan(a) ? (b_null ? a : bv) : (b_null ? a : fmaxf(a, bv));
-    if (isnan(r) && live) atomicMin(err, ugvc_pack_error(rec, cb.feature, REASON_NULL_FEATURE));
-    a = r;
-}
 
 // NCH trees at once from the heap form in shared memory: node = (threshold bits, byte offset of the feature's row in
 // the thread's tile column).  All indices are kept as byte offsets so that a level costs six instructions per chain:
