@@ -297,6 +297,55 @@ int ugvc_filter_bgzf(ugvc_ctx* ctx, int lane, const uint8_t* bgzf, size_t n_byte
                      double threshold, int flags, uint8_t* out_bgzf, size_t out_capacity, size_t* out_bytes,
                      uint32_t* out_block_csize, size_t block_capacity, size_t* out_n_blocks, ugvc_recinfo* out_recinfo,
                      int64_t* out_line_start, uint8_t* out_low_score, size_t capacity_records, int64_t* out_n_records);
+/* ugvc_filter_bgzf with the rest of the tool's record edits, so that every run but --treat_multiallelics can stay on
+ * the device (ugvc_filter_bgzf is this call with with_model = 1 and everything else zero):
+ *   with_model = 0     a model-less plan (FILTER keeps its non-empty pieces, PASS when none is left; no TREE_SCORE;
+ *                      QUAL untouched; out_low_score all 0)
+ *   recalibrate_genotype  --recalibrate_genotype (filter_variants_pipeline.py:203-215): GQ = int(second smallest -
+ *                      smallest phred), PL = int() of the first min(n_classes, n_alleles (n_alleles + 1) / 2) phreds,
+ *                      GT = genotype of the first smallest PL ('|' when the input GT is phased), on the first sample only,
+ *                      missing keys appended in the order GQ, PL, GT; no TREE_SCORE; UGVC_FILE_OVERWRITE_QUAL writes
+ *                      %g of the GQ difference to QUAL.  Needs a model and ugvc_enable_phreds(ctx, 1) before ugvc_reserve.
+ *   blacklists         Blacklist.apply with selection_fcn = ALL for the range's contig: blacklist k is the sorted POS
+ *                      array blacklist_pos[blacklist_pos_off[k], blacklist_pos_off[k + 1]) and the annotation
+ *                      blacklist_names[blacklist_name_off[k], ..[k + 1]).  INFO gets BLACKLST= and the non-PASS
+ *                      annotations of the record joined with ',', the CG flag (UGVC_FILE_BLACKLIST_CG) first, then the
+ *                      blacklists in order.  At most UGVC_MAX_BLACKLISTS blacklists, UGVC_MAX_BLACKLIST_POSITIONS
+ *                      positions and UGVC_MAX_BLACKLIST_NAME_BYTES of annotations a call (UGVC_E_ARG beyond).
+ *   out_end            (may be NULL; capacity_records entries) INFO/END of every record, 0 where there is none: the
+ *                      rule of ugvc_info_end, read while the INFO column is copied.
+ *   n_blacklisted      (out) records with at least one annotation, CG included.
+ * UGVC_E_FALLBACK as for ugvc_filter_bgzf, and also for a recalibrated record whose phreds are not finite or whose int()
+ * leaves int32 (or a model with fewer than two classes), for a GQ that %g prints in exponent form under
+ * UGVC_FILE_OVERWRITE_QUAL, and for edited text that outgrows the writer's buffer (long annotations).  Output bytes
+ * equal ugvc_splice_records' on the same records. */
+#define UGVC_MAX_BLACKLISTS 31
+#define UGVC_MAX_BLACKLIST_POSITIONS (1ll << 28)
+#define UGVC_MAX_BLACKLIST_NAME_BYTES 4096
+typedef struct ugvc_file_edits {
+    int with_model;
+    int recalibrate_genotype;
+    int n_blacklists;
+    const int64_t* blacklist_pos;
+    const int64_t* blacklist_pos_off;   /* n_blacklists + 1 entries, from 0 */
+    const char* blacklist_names;
+    const int64_t* blacklist_name_off;  /* n_blacklists + 1 entries, from 0 */
+    int64_t* out_end;
+    int64_t n_blacklisted;
+} ugvc_file_edits;
+int ugvc_filter_bgzf_edits(ugvc_ctx* ctx, int lane, const uint8_t* bgzf, size_t n_bytes, uint32_t skip_head, uint64_t take_bytes,
+                           double threshold, int flags, ugvc_file_edits* edits, uint8_t* out_bgzf, size_t out_capacity,
+                           size_t* out_bytes, uint32_t* out_block_csize, size_t block_capacity, size_t* out_n_blocks,
+                           ugvc_recinfo* out_recinfo, int64_t* out_line_start, uint8_t* out_low_score, size_t capacity_records,
+                           int64_t* out_n_records);
+/* Test hook: the record writer of ugvc_filter_bgzf_edits alone, on the caller's records (text, line_start and recinfo as
+ * ugvc_filter_batch returns them), scores (low_score / qual, with_model) and phreds ([n][n_classes],
+ * recalibrate_genotype), staged in lane 0.  Returns the bytes of the edited text written to out (out_line_start: n + 1
+ * entries; edits->out_end filled when given), UGVC_E_FALLBACK when the device writer hands the records back. */
+int64_t ugvc_test_write_records(ugvc_ctx* ctx, const uint8_t* text, size_t n_bytes, const int64_t* line_start,
+                                const ugvc_recinfo* recinfo, int64_t n, const uint8_t* low_score, const double* qual,
+                                const double* phreds, int n_classes, int flags, ugvc_file_edits* edits, uint8_t* out,
+                                size_t capacity, int64_t* out_line_start);
 /* Stage seconds of the last ugvc_filter_bgzf call on `lane`: H2D + inflate, K1..K3, record writer, deflate + pack,
  * D2H (device-timed with CUDA events). */
 int ugvc_filter_bgzf_stage_ms(ugvc_ctx* ctx, int lane, float out_ms[5]);

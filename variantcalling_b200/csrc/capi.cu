@@ -54,6 +54,14 @@ struct Lane {
         uint8_t* d_packed = nullptr;
         int* d_fallback = nullptr;
         int* h_fallback = nullptr;      // pinned
+        uint32_t* d_bl_mask = nullptr;  // [cap_records]: annotation bits of each record
+        int64_t* d_end = nullptr;       // [cap_records]: INFO/END of each record
+        unsigned long long* d_n_bl = nullptr;
+        unsigned long long* h_n_bl = nullptr;  // pinned
+        // blacklists of the current call (ugvc_filter_bgzf_edits), grown on demand up to UGVC_MAX_BLACKLIST_POSITIONS
+        int64_t* d_bl_pos = nullptr;
+        size_t cap_bl_pos = 0;
+        uint8_t* d_bl_meta = nullptr;   // position offsets, name offsets, names (FIO_BL_META bytes)
         int64_t* h_total = nullptr;     // pinned
         std::vector<uint32_t> h_bsize;
         cudaEvent_t ev[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
@@ -170,6 +178,12 @@ static void free_lane(Lane& l) {
     cudaFree(l.fb.d_packed);
     cudaFree(l.fb.d_fallback);
     if (l.fb.h_fallback) cudaFreeHost(l.fb.h_fallback);
+    cudaFree(l.fb.d_bl_mask);
+    cudaFree(l.fb.d_end);
+    cudaFree(l.fb.d_n_bl);
+    if (l.fb.h_n_bl) cudaFreeHost(l.fb.h_n_bl);
+    cudaFree(l.fb.d_bl_pos);
+    cudaFree(l.fb.d_bl_meta);
     if (l.fb.h_total) cudaFreeHost(l.fb.h_total);
     for (auto& e : l.fb.ev)
         if (e) cudaEventDestroy(e);
@@ -1318,6 +1332,16 @@ extern "C" int ugvc_filter_bgzf(ugvc_ctx* ctx, int, const uint8_t*, size_t, uint
                                 uint32_t*, size_t, size_t*, ugvc_recinfo*, int64_t*, uint8_t*, size_t, int64_t*) {
     return fail(ctx, UGVC_E_FALLBACK, "the device-side record writer is not part of the host emulation");
 }
+extern "C" int ugvc_filter_bgzf_edits(ugvc_ctx* ctx, int, const uint8_t*, size_t, uint32_t, uint64_t, double, int,
+                                      ugvc_file_edits*, uint8_t*, size_t, size_t*, uint32_t*, size_t, size_t*, ugvc_recinfo*,
+                                      int64_t*, uint8_t*, size_t, int64_t*) {
+    return fail(ctx, UGVC_E_FALLBACK, "the device-side record writer is not part of the host emulation");
+}
+extern "C" int64_t ugvc_test_write_records(ugvc_ctx* ctx, const uint8_t*, size_t, const int64_t*, const ugvc_recinfo*, int64_t,
+                                       const uint8_t*, const double*, const double*, int, int, ugvc_file_edits*, uint8_t*, size_t,
+                                       int64_t*) {
+    return fail(ctx, UGVC_E_STATE, "the device-side record writer is not part of the host emulation");
+}
 extern "C" int ugvc_filter_bgzf_stage_ms(ugvc_ctx*, int, float*) { return UGVC_E_STATE; }
 extern "C" int ugvc_filter_bgzf_first_records(ugvc_ctx*, int, const uint64_t*, int, int64_t*) { return UGVC_E_STATE; }
 extern "C" int ugvc_test_device_deflate(ugvc_ctx* ctx, const uint8_t*, size_t, int, uint8_t*, size_t, uint32_t*, size_t, size_t*,
@@ -1325,6 +1349,8 @@ extern "C" int ugvc_test_device_deflate(ugvc_ctx* ctx, const uint8_t*, size_t, i
     return fail(ctx, UGVC_E_STATE, "the device BGZF encoder is not part of the host emulation");
 }
 #else
+#define FIO_BL_NAMES_AT (8 * (UGVC_MAX_BLACKLISTS + 1) + 4 * (UGVC_MAX_BLACKLISTS + 2))
+#define FIO_BL_META (FIO_BL_NAMES_AT + UGVC_MAX_BLACKLIST_NAME_BYTES)
 static int file_bufs(ugvc_ctx* ctx, Lane& l) {
     Lane::FileBufs& f = l.fb;
     if (f.d_out_text) return UGVC_OK;
@@ -1347,6 +1373,11 @@ static int file_bufs(ugvc_ctx* ctx, Lane& l) {
     CU(cudaMalloc(&f.d_packed, f.cap_blocks * (size_t)DEF_BLOCK_STRIDE));
     CU(cudaMalloc(&f.d_fallback, sizeof(int)));
     CU(cudaHostAlloc(&f.h_fallback, sizeof(int), cudaHostAllocDefault));
+    CU(cudaMalloc(&f.d_bl_mask, (cap_rec ? cap_rec : 1) * sizeof(uint32_t)));
+    CU(cudaMalloc(&f.d_end, (cap_rec ? cap_rec : 1) * sizeof(int64_t)));
+    CU(cudaMalloc(&f.d_n_bl, sizeof(unsigned long long)));
+    CU(cudaHostAlloc(&f.h_n_bl, sizeof(unsigned long long), cudaHostAllocDefault));
+    CU(cudaMalloc(&f.d_bl_meta, FIO_BL_META));
     CU(cudaHostAlloc(&f.h_total, sizeof(int64_t), cudaHostAllocDefault));
     for (auto& e : f.ev) CU(cudaEventCreate(&e));
     return def_tables(ctx);
@@ -1377,23 +1408,140 @@ static int encode_blocks(ugvc_ctx* ctx, Lane::FileBufs& f, size_t n_text, int n_
     return UGVC_OK;
 }
 
-extern "C" int ugvc_filter_bgzf(ugvc_ctx* ctx, int lane, const uint8_t* bgzf, size_t n_bytes, uint32_t skip_head, uint64_t take_bytes,
-                                double threshold, int flags, uint8_t* out_bgzf, size_t out_capacity, size_t* out_bytes,
-                                uint32_t* out_block_csize, size_t block_capacity, size_t* out_n_blocks, ugvc_recinfo* out_recinfo,
-                                int64_t* out_line_start, uint8_t* out_low_score, size_t capacity_records, int64_t* out_n_records) {
+// The blacklists of a call to the device: positions (grown on demand), and one small block of position offsets, value
+// offsets and value texts.  A value is the annotation's ';'-separated pieces without the empty and PASS ones, joined
+// with ',' -- what the host writer makes of the ';'-joined code string (hostio.cpp splice_one), so that the kernels only
+// join whole values.
+static int upload_blacklists(ugvc_ctx* ctx, Lane::FileBufs& f, const ugvc_file_edits& e, FioEdits& ed, cudaStream_t st) {
+    ed.n_bl = e.n_blacklists;
+    if (e.n_blacklists == 0) return UGVC_OK;
+    if (e.n_blacklists < 0 || e.n_blacklists > UGVC_MAX_BLACKLISTS)
+        return fail(ctx, UGVC_E_ARG, "filter_bgzf_edits: more blacklists than the annotation code holds (" +
+                                         std::to_string(UGVC_MAX_BLACKLISTS) + ")");
+    if (!e.blacklist_pos_off || !e.blacklist_name_off || (!e.blacklist_names && e.blacklist_name_off[e.n_blacklists]))
+        return fail(ctx, UGVC_E_ARG, "filter_bgzf_edits: NULL blacklist table");
+    const int nb = e.n_blacklists;
+    if (e.blacklist_pos_off[0] != 0 || e.blacklist_name_off[0] != 0)
+        return fail(ctx, UGVC_E_ARG, "filter_bgzf_edits: blacklist offsets must start at 0");
+    for (int k = 0; k < nb; ++k)
+        if (e.blacklist_pos_off[k + 1] < e.blacklist_pos_off[k] || e.blacklist_name_off[k + 1] < e.blacklist_name_off[k])
+            return fail(ctx, UGVC_E_ARG, "filter_bgzf_edits: blacklist offsets must not decrease");
+    const int64_t n_pos = e.blacklist_pos_off[nb];
+    if (n_pos > (int64_t)UGVC_MAX_BLACKLIST_POSITIONS)
+        return fail(ctx, UGVC_E_ARG, "filter_bgzf_edits: more blacklist positions than UGVC_MAX_BLACKLIST_POSITIONS");
+    if (n_pos && !e.blacklist_pos) return fail(ctx, UGVC_E_ARG, "filter_bgzf_edits: NULL blacklist positions");
+    for (int k = 0; k < nb; ++k)
+        for (int64_t j = e.blacklist_pos_off[k] + 1; j < e.blacklist_pos_off[k + 1]; ++j)
+            if (e.blacklist_pos[j] < e.blacklist_pos[j - 1])
+                return fail(ctx, UGVC_E_ARG, "filter_bgzf_edits: blacklist " + std::to_string(k) + "'s positions are not sorted");
+    std::vector<uint8_t> meta(FIO_BL_META, 0);
+    int64_t* pos_off = reinterpret_cast<int64_t*>(meta.data());
+    int32_t* name_off = reinterpret_cast<int32_t*>(meta.data() + 8 * (UGVC_MAX_BLACKLISTS + 1));
+    uint8_t* names = meta.data() + FIO_BL_NAMES_AT;
+    size_t at = 0;
+    for (int k = 0; k < nb; ++k) {
+        pos_off[k] = e.blacklist_pos_off[k];
+        name_off[k] = (int32_t)at;
+        const char* v = e.blacklist_names + e.blacklist_name_off[k];
+        const size_t vl = (size_t)(e.blacklist_name_off[k + 1] - e.blacklist_name_off[k]);
+        bool first = true;
+        size_t p0 = 0;
+        for (size_t q = 0; q <= vl; ++q) {
+            if (q < vl && v[q] != ';') continue;
+            const size_t pl = q - p0;
+            if (pl && !(pl == 4 && memcmp(v + p0, "PASS", 4) == 0)) {
+                if (at + pl + 1 > UGVC_MAX_BLACKLIST_NAME_BYTES)
+                    return fail(ctx, UGVC_E_ARG, "filter_bgzf_edits: blacklist annotations longer than UGVC_MAX_BLACKLIST_NAME_BYTES");
+                if (!first) names[at++] = ',';
+                memcpy(names + at, v + p0, pl);
+                at += pl;
+                first = false;
+            }
+            p0 = q + 1;
+        }
+    }
+    pos_off[nb] = n_pos;
+    name_off[nb] = (int32_t)at;
+    if ((size_t)n_pos > f.cap_bl_pos) {
+        CU(cudaStreamSynchronize(st));
+        cudaFree(f.d_bl_pos);
+        f.d_bl_pos = nullptr;
+        f.cap_bl_pos = 0;
+        CU(cudaMalloc(&f.d_bl_pos, (size_t)n_pos * sizeof(int64_t)));
+        f.cap_bl_pos = (size_t)n_pos;
+    }
+    if (n_pos) CU(cudaMemcpyAsync(f.d_bl_pos, e.blacklist_pos, (size_t)n_pos * sizeof(int64_t), cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(f.d_bl_meta, meta.data(), FIO_BL_META, cudaMemcpyHostToDevice, st));
+    CU(cudaStreamSynchronize(st));  // `meta` is this function's
+    ed.bl_pos = f.d_bl_pos;
+    ed.bl_pos_off = reinterpret_cast<const int64_t*>(f.d_bl_meta);
+    ed.bl_name_off = reinterpret_cast<const int32_t*>(f.d_bl_meta + 8 * (UGVC_MAX_BLACKLISTS + 1));
+    ed.bl_name = f.d_bl_meta + FIO_BL_NAMES_AT;
+    return UGVC_OK;
+}
+
+// The record writer on records already on the device (text, K1's line starts and recinfo, K3's low_score / qual): lengths,
+// scan, copy into f.d_out_text (16 zero bytes after it), *out_text = its length.  UGVC_E_FALLBACK when a record needs the
+// host writer (splice_len's flag) or the edited text outgrows the writer's buffer (long blacklist annotations); the copy
+// pass's own flag lands in *f.h_fallback, read by the caller after its next synchronise.
+static int write_records(ugvc_ctx* ctx, Lane::FileBufs& f, const uint8_t* d_text, const int64_t* d_line_start,
+                         const ugvc_recinfo* d_recinfo, const uint8_t* d_low, const double* d_qual, int64_t n, const FioEdits& ed,
+                         cudaStream_t st, size_t* out_text) {
+    CU(cudaMemsetAsync(f.d_fallback, 0, sizeof(int), st));
+    CU(cudaMemsetAsync(f.d_n_bl, 0, sizeof(unsigned long long), st));
+    CU(cudaMemsetAsync(f.d_len + n, 0, sizeof(int64_t), st));
+    fio_launch_splice_len(d_text, d_line_start, d_recinfo, d_low, d_qual, n, ed, f.d_len, f.d_score, f.d_fallback, ctx->sm_count, st);
+    size_t tmp = f.scan_tmp_bytes;
+    CU(fio_scan_i64(f.d_scan_tmp, tmp, f.d_len, f.d_out_ls, n + 1, st));
+    CU(cudaMemcpyAsync(f.h_total, f.d_out_ls + n, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(f.h_fallback, f.d_fallback, sizeof(int), cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(f.h_n_bl, f.d_n_bl, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    if (*f.h_fallback) return UGVC_E_FALLBACK;
+    *out_text = (size_t)*f.h_total;
+    if (*out_text > f.cap_out) return fail(ctx, UGVC_E_FALLBACK, "filter_bgzf: the edited text exceeds the writer's buffer");
+    fio_launch_splice_copy(d_text, d_line_start, d_recinfo, d_low, n, ed, f.d_out_ls, f.d_score, f.d_out_text, f.d_fallback,
+                           ctx->sm_count, st);
+    CU(cudaMemsetAsync(f.d_out_text + *out_text, 0, 16, st));  // the encoder reads whole words
+    CU(cudaMemcpyAsync(f.h_fallback, f.d_fallback, sizeof(int), cudaMemcpyDeviceToHost, st));
+    return UGVC_OK;
+}
+
+extern "C" int ugvc_filter_bgzf_edits(ugvc_ctx* ctx, int lane, const uint8_t* bgzf, size_t n_bytes, uint32_t skip_head,
+                                      uint64_t take_bytes, double threshold, int flags, ugvc_file_edits* edits, uint8_t* out_bgzf,
+                                      size_t out_capacity, size_t* out_bytes, uint32_t* out_block_csize, size_t block_capacity,
+                                      size_t* out_n_blocks, ugvc_recinfo* out_recinfo, int64_t* out_line_start,
+                                      uint8_t* out_low_score, size_t capacity_records, int64_t* out_n_records) {
     if (!ctx) return UGVC_E_ARG;
+    if (!edits) return fail(ctx, UGVC_E_ARG, "filter_bgzf_edits: NULL edits");
+    const ugvc_file_edits& e = *edits;
+    edits->n_blacklisted = 0;
     if (!ctx->has_plan || ctx->lanes.empty()) return fail(ctx, UGVC_E_STATE, "filter_bgzf: load a plan and reserve first");
-    if (ctx->plan.h.model_kind == MODEL_NONE) return fail(ctx, UGVC_E_STATE, "filter_bgzf: the plan carries no model");
+    if (e.with_model && ctx->plan.h.model_kind == MODEL_NONE) return fail(ctx, UGVC_E_STATE, "filter_bgzf: the plan carries no model");
+    if (e.recalibrate_genotype && !e.with_model)
+        return fail(ctx, UGVC_E_ARG, "filter_bgzf_edits: recalibrate_genotype needs with_model");
     if (lane < 0 || lane >= (int)ctx->lanes.size()) return fail(ctx, UGVC_E_ARG, "filter_bgzf: lane out of range");
     if (!bgzf || !n_bytes || !out_bgzf || !out_bytes || !out_n_records) return fail(ctx, UGVC_E_ARG, "filter_bgzf: NULL argument");
     CU(cudaSetDevice(ctx->device));
     Lane& l = ctx->lanes[lane];
     if (l.submitted) return fail(ctx, UGVC_E_STATE, "filter_bgzf: lane already has a batch in flight");
+    if (e.recalibrate_genotype && (ctx->want_phreds != 1 || !l.b.phreds))
+        return fail(ctx, UGVC_E_STATE, "filter_bgzf_edits: recalibrate_genotype needs ugvc_enable_phreds(ctx, 1) before ugvc_reserve");
     int rc = file_bufs(ctx, l);
     if (rc) return rc;
     Lane::FileBufs& f = l.fb;
     cudaStream_t st = l.stream;
     (void)cudaGetLastError();  // nothing stale from this host thread's earlier calls
+    FioEdits ed{};
+    ed.with_model = e.with_model ? 1 : 0;
+    ed.flags = flags;
+    ed.phreds = e.recalibrate_genotype ? l.b.phreds : nullptr;
+    ed.n_classes = ctx->plan.h.n_classes;
+    ed.bl_mask = f.d_bl_mask;
+    ed.n_blacklisted = f.d_n_bl;
+    ed.out_end = e.out_end ? f.d_end : nullptr;
+    rc = upload_blacklists(ctx, f, e, ed, st);
+    if (rc) return rc;
     CU(cudaEventRecord(f.ev[0], st));
     // ---- compressed blocks -> text on the device, the range's first byte 16-byte aligned
     const size_t shift = (16 - (skip_head & 15u)) & 15u;
@@ -1425,22 +1573,9 @@ extern "C" int ugvc_filter_bgzf(ugvc_ctx* ctx, int lane, const uint8_t* bgzf, si
     *out_n_records = n;
     if ((size_t)n > capacity_records) return fail(ctx, UGVC_E_ARG, "filter_bgzf: output capacity smaller than the record count");
     // ---- record writer
-    CU(cudaMemsetAsync(f.d_fallback, 0, sizeof(int), st));
-    CU(cudaMemsetAsync(f.d_len + n, 0, sizeof(int64_t), st));
-    fio_launch_splice_len(d_text, l.b.line_start, l.b.recinfo, l.b.low_score, l.b.qual, n, flags, f.d_len, f.d_score, f.d_fallback,
-                          ctx->sm_count, st);
-    size_t tmp = f.scan_tmp_bytes;
-    CU(fio_scan_i64(f.d_scan_tmp, tmp, f.d_len, f.d_out_ls, n + 1, st));
-    CU(cudaMemcpyAsync(f.h_total, f.d_out_ls + n, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
-    CU(cudaMemcpyAsync(f.h_fallback, f.d_fallback, sizeof(int), cudaMemcpyDeviceToHost, st));
-    CU(cudaStreamSynchronize(st));
-    if (*f.h_fallback) return UGVC_E_FALLBACK;
-    const size_t out_text = (size_t)*f.h_total;
-    if (out_text > f.cap_out) return fail(ctx, UGVC_E_ARG, "filter_bgzf: the edited text exceeds the writer's buffer");
-    fio_launch_splice_copy(d_text, l.b.line_start, l.b.recinfo, l.b.low_score, n, flags, f.d_out_ls, f.d_score, f.d_out_text,
-                           f.d_fallback, ctx->sm_count, st);
-    CU(cudaMemsetAsync(f.d_out_text + out_text, 0, 16, st));  // the encoder reads whole words
-    CU(cudaMemcpyAsync(f.h_fallback, f.d_fallback, sizeof(int), cudaMemcpyDeviceToHost, st));
+    size_t out_text = 0;
+    rc = write_records(ctx, f, d_text, l.b.line_start, l.b.recinfo, l.b.low_score, l.b.qual, n, ed, st, &out_text);
+    if (rc) return rc;
     CU(cudaEventRecord(f.ev[3], st));
     // ---- deflate, pack
     const int n_blocks = (int)((out_text + DEF_CHUNK - 1) / DEF_CHUNK);
@@ -1463,13 +1598,95 @@ extern "C" int ugvc_filter_bgzf(ugvc_ctx* ctx, int lane, const uint8_t* bgzf, si
     if (out_block_csize && n_blocks) memcpy(out_block_csize, f.h_bsize.data(), (size_t)n_blocks * sizeof(uint32_t));
     if (out_recinfo && n) CU(cudaMemcpyAsync(out_recinfo, l.b.recinfo, (size_t)n * sizeof(ugvc_recinfo), cudaMemcpyDeviceToHost, st));
     if (out_line_start) CU(cudaMemcpyAsync(out_line_start, f.d_out_ls, (size_t)(n + 1) * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
-    if (out_low_score && n) CU(cudaMemcpyAsync(out_low_score, l.b.low_score, (size_t)n, cudaMemcpyDeviceToHost, st));
+    if (out_low_score && n) {
+        if (e.with_model) CU(cudaMemcpyAsync(out_low_score, l.b.low_score, (size_t)n, cudaMemcpyDeviceToHost, st));
+        else memset(out_low_score, 0, (size_t)n);  // no score: nothing is LOW_SCORE
+    }
+    if (e.out_end && n) CU(cudaMemcpyAsync(e.out_end, f.d_end, (size_t)n * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
     CU(cudaEventRecord(f.ev[5], st));
     CU(cudaStreamSynchronize(st));
     *out_bytes = packed;
+    edits->n_blacklisted = (int64_t)*f.h_n_bl;
     if (out_n_blocks) *out_n_blocks = (size_t)n_blocks;
     for (int k = 0; k < 5; ++k) cudaEventElapsedTime(&f.ms[k], f.ev[k], f.ev[k + 1]);
     return UGVC_OK;
+}
+
+extern "C" int ugvc_filter_bgzf(ugvc_ctx* ctx, int lane, const uint8_t* bgzf, size_t n_bytes, uint32_t skip_head, uint64_t take_bytes,
+                                double threshold, int flags, uint8_t* out_bgzf, size_t out_capacity, size_t* out_bytes,
+                                uint32_t* out_block_csize, size_t block_capacity, size_t* out_n_blocks, ugvc_recinfo* out_recinfo,
+                                int64_t* out_line_start, uint8_t* out_low_score, size_t capacity_records, int64_t* out_n_records) {
+    ugvc_file_edits e{};  // a model, no blacklists, no genotype recalibration, no INFO/END
+    e.with_model = 1;
+    return ugvc_filter_bgzf_edits(ctx, lane, bgzf, n_bytes, skip_head, take_bytes, threshold, flags, &e, out_bgzf, out_capacity,
+                                  out_bytes, out_block_csize, block_capacity, out_n_blocks, out_recinfo, out_line_start,
+                                  out_low_score, capacity_records, out_n_records);
+}
+
+extern "C" int64_t ugvc_test_write_records(ugvc_ctx* ctx, const uint8_t* text, size_t n_bytes, const int64_t* line_start,
+                                       const ugvc_recinfo* recinfo, int64_t n, const uint8_t* low_score, const double* qual,
+                                       const double* phreds, int n_classes, int flags, ugvc_file_edits* edits, uint8_t* out,
+                                       size_t capacity, int64_t* out_line_start) {
+    // test hook: the record writer of ugvc_filter_bgzf_edits on the caller's records, K1's recinfo and the caller's scores
+    // and phreds (so that every FORMAT shape, allele count and phred -- ties, NaN, beyond int32 -- can be put to it),
+    // staged in lane 0's buffers
+    if (!ctx || !edits || n < 0 || !text || !line_start || !recinfo || !out || !out_line_start) return UGVC_E_ARG;
+    if (ctx->lanes.empty()) return fail(ctx, UGVC_E_STATE, "test_write_records: reserve first (the records go to lane 0)");
+    const ugvc_file_edits& e = *edits;
+    edits->n_blacklisted = 0;
+    if ((e.with_model && (!low_score || !qual)) || (e.recalibrate_genotype && (!e.with_model || !phreds || n_classes < 0)))
+        return fail(ctx, UGVC_E_ARG, "test_write_records: scores / phreds missing");
+    CU(cudaSetDevice(ctx->device));
+    Lane& l = ctx->lanes[0];
+    if (l.submitted) return fail(ctx, UGVC_E_STATE, "test_write_records: lane 0 has a batch in flight");
+    if ((size_t)n > l.b.cap_records || n_bytes > ctx->cap_bytes) return fail(ctx, UGVC_E_ARG, "test_write_records: larger than reserved");
+    int rc = file_bufs(ctx, l);
+    if (rc) return rc;
+    Lane::FileBufs& f = l.fb;
+    cudaStream_t st = l.stream;
+    (void)cudaGetLastError();
+    struct DevFree {
+        void* p = nullptr;
+        ~DevFree() { cudaFree(p); }
+    } d_ph, d_low, d_qual;
+    const size_t nn = n ? (size_t)n : 1;
+    CU(cudaMemcpyAsync(l.d_text, text, n_bytes, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(l.b.line_start, line_start, (nn + 1) * sizeof(int64_t), cudaMemcpyHostToDevice, st));
+    if (n) CU(cudaMemcpyAsync(l.b.recinfo, recinfo, (size_t)n * sizeof(ugvc_recinfo), cudaMemcpyHostToDevice, st));
+    CU(cudaMalloc(&d_low.p, nn));
+    CU(cudaMalloc(&d_qual.p, nn * sizeof(double)));
+    CU(cudaMemsetAsync(d_low.p, 0, nn, st));
+    CU(cudaMemsetAsync(d_qual.p, 0, nn * sizeof(double), st));
+    if (low_score && n) CU(cudaMemcpyAsync(d_low.p, low_score, (size_t)n, cudaMemcpyHostToDevice, st));
+    if (qual && n) CU(cudaMemcpyAsync(d_qual.p, qual, (size_t)n * sizeof(double), cudaMemcpyHostToDevice, st));
+    FioEdits ed{};
+    ed.with_model = e.with_model ? 1 : 0;
+    ed.flags = flags;
+    ed.n_classes = n_classes;
+    if (e.recalibrate_genotype) {
+        const size_t np = nn * (size_t)(n_classes > 0 ? n_classes : 1);
+        CU(cudaMalloc(&d_ph.p, np * sizeof(double)));
+        if (n && n_classes > 0) CU(cudaMemcpyAsync(d_ph.p, phreds, (size_t)n * n_classes * sizeof(double), cudaMemcpyHostToDevice, st));
+        ed.phreds = static_cast<const double*>(d_ph.p);
+    }
+    ed.bl_mask = f.d_bl_mask;
+    ed.n_blacklisted = f.d_n_bl;
+    ed.out_end = e.out_end ? f.d_end : nullptr;
+    rc = upload_blacklists(ctx, f, e, ed, st);
+    if (rc) return rc;
+    size_t out_text = 0;
+    rc = write_records(ctx, f, l.d_text, l.b.line_start, l.b.recinfo, static_cast<const uint8_t*>(d_low.p),
+                       static_cast<const double*>(d_qual.p), n, ed, st, &out_text);
+    if (rc) return rc;
+    CU(cudaStreamSynchronize(st));
+    if (*f.h_fallback) return UGVC_E_FALLBACK;
+    if (out_text > capacity) return fail(ctx, UGVC_E_ARG, "test_write_records: capacity smaller than the edited text");
+    if (out_text) CU(cudaMemcpyAsync(out, f.d_out_text, out_text, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(out_line_start, f.d_out_ls, (nn + 1) * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    if (e.out_end && n) CU(cudaMemcpyAsync(e.out_end, f.d_end, (size_t)n * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    edits->n_blacklisted = (int64_t)*f.h_n_bl;
+    return (int64_t)out_text;
 }
 
 extern "C" int ugvc_filter_bgzf_stage_ms(ugvc_ctx* ctx, int lane, float out_ms[5]) {

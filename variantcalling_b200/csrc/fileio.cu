@@ -4,11 +4,14 @@
 // filter_variants_pipeline.py:188-228) and the round-1 tool did the same edit on host threads
 // (hostio.cpp: ugvc_splice_records) followed by zlib.  Here the edited text never exists on the host:
 //   splice_len    one thread per record: length of the edited line (new FILTER column, ";TREE_SCORE=<%g>", the
-//                 optional CG blacklist annotation, the optional QUAL overwrite)
+//                 BLACKLST annotations -- the CG flag and a binary search of POS in each blacklist --, the optional
+//                 QUAL overwrite, the recalibrated GT / GQ / PL of the first sample)
 //   (exclusive scan of the lengths -> out_line_start)
-//   splice_copy   one warp per record: the pieces are copied with consecutive lanes on consecutive bytes;
-//                 anything the simple INFO rule does not cover (an existing TREE_SCORE= / BLACKLST= key, empty
-//                 INFO pieces, a "." INFO) raises a flag and the caller falls back to the host writer
+//   splice_copy   one warp per record: the pieces are copied with consecutive lanes on consecutive bytes, the short
+//                 rewritten ones (FILTER, BLACKLST, the first sample) by lane 0 with the routine that measured them;
+//                 INFO/END is picked up on the way.  Anything the simple INFO rule does not cover (an existing
+//                 TREE_SCORE= / BLACKLST= key, empty INFO pieces, a "." INFO) raises a flag and the caller falls back
+//                 to the host writer
 //   deflate       one thread per 56 KiB of output text -> one BGZF block (deflate.cuh), then the blocks are
 //                 packed back to back
 // Same text as the host writer produces (tests compare the two), so the output contract is unchanged.
@@ -138,8 +141,6 @@ __device__ uint32_t fio_filter(const uint8_t* fp, uint32_t fl, bool low, uint8_t
     return n;
 }
 
-#define FIO_CG_TEXT ";BLACKLST=CG_NON_HMER_INDEL"
-#define FIO_CG_LEN 27u
 #define FIO_SCORE_KEY ";TREE_SCORE="
 #define FIO_SCORE_KEY_LEN 12u
 
@@ -161,15 +162,231 @@ __device__ __forceinline__ FioRec fio_rec(const int64_t* line_start, const ugvc_
     return r;
 }
 
+// ---- small writers: out == nullptr only counts, so that the length pass and the copy pass share one routine
+__device__ __forceinline__ uint32_t fio_put(uint8_t* out, uint32_t n, const uint8_t* src, uint32_t len) {
+    if (out)
+        for (uint32_t k = 0; k < len; ++k) out[n + k] = src[k];
+    return n + len;
+}
+__device__ __forceinline__ uint32_t fio_putc(uint8_t* out, uint32_t n, uint8_t c) {
+    if (out) out[n] = c;
+    return n + 1;
+}
+__device__ uint32_t fio_put_int(uint8_t* out, uint32_t n, int v) {  // std::to_string(int)
+    char d[10];
+    int k = 0;
+    uint32_t u = v < 0 ? 0u - (uint32_t)v : (uint32_t)v;
+    do {
+        d[k++] = (char)('0' + u % 10u);
+        u /= 10u;
+    } while (u);
+    if (v < 0) n = fio_putc(out, n, '-');
+    while (k) n = fio_putc(out, n, (uint8_t)d[--k]);
+    return n;
+}
+
+// ---- BLACKLST: ";BLACKLST=" and the ','-joined values of the record's annotation bits in merge order (bit 0: the CG
+// insertion flag, bit k + 1: blacklist k), values that are empty skipped, nothing at all when no value is left
+// (hostio.cpp splice_one; the host side of ugvc_filter_bgzf_edits already dropped the PASS / empty pieces of each value)
+__device__ uint32_t fio_blacklst(uint32_t mask, int n_bl, const uint8_t* bl_name, const int32_t* bl_name_off, uint8_t* out) {
+    uint32_t n = 0;
+    bool any = false;
+    for (int k = 0; k <= n_bl; ++k) {
+        if (!((mask >> k) & 1u)) continue;
+        const uint8_t* v = reinterpret_cast<const uint8_t*>("CG_NON_HMER_INDEL");
+        uint32_t vl = 17;
+        if (k) {
+            v = bl_name + bl_name_off[k - 1];
+            vl = (uint32_t)(bl_name_off[k] - bl_name_off[k - 1]);
+        }
+        if (!vl) continue;
+        n = any ? fio_putc(out, n, ',') : fio_put(out, n, reinterpret_cast<const uint8_t*>(";BLACKLST="), 10);
+        any = true;
+        n = fio_put(out, n, v, vl);
+    }
+    return n;
+}
+
+// the annotation bits of a record: the CG flag of K1 under UGVC_FILE_BLACKLIST_CG, then a binary search of POS in each
+// blacklist's sorted positions (Blacklist.apply with selection_fcn = ALL: a (chrom, pos) set; the caller uploads the
+// positions of the range's contig)
+__device__ uint32_t fio_bl_mask(int64_t pos, bool cg, int n_bl, const int64_t* bl_pos, const int64_t* bl_pos_off) {
+    uint32_t mask = cg ? 1u : 0u;
+    for (int k = 0; k < n_bl; ++k) {
+        int64_t lo = bl_pos_off[k], hi = bl_pos_off[k + 1];
+        while (lo < hi) {
+            const int64_t mid = (lo + hi) >> 1;
+            if (bl_pos[mid] < pos) lo = mid + 1;
+            else hi = mid;
+        }
+        if (lo < bl_pos_off[k + 1] && bl_pos[lo] == pos) mask |= 2u << k;
+    }
+    return mask;
+}
+
+// ---- --recalibrate_genotype (hostio.cpp splice_one / recalibrated_sample): GQ = int(second smallest - smallest) of the
+// n_classes phreds, PL = int() of the first min(n_classes, na (na + 1) / 2) of them (at least one), GT = the genotype of
+// the first smallest PL (gt_from_pl_idx).  false: a phred that is not finite or whose int() would leave int32 -- the
+// record is left to the host writer.
+struct FioGeno {
+    const double* ph;
+    double gq;  // QUAL under UGVC_FILE_OVERWRITE_QUAL prints this, not int(gq)
+    int n_pl, a, b;
+};
+__device__ bool fio_geno(const double* ph, int n_classes, uint32_t recflags, FioGeno& g) {
+    if (n_classes < 2) return false;
+    for (int k = 0; k < n_classes; ++k)
+        if (!(fabs(ph[k]) < 2147483647.0)) return false;
+    double m1 = ph[0], m2 = ph[1];
+    if (m2 < m1) {
+        const double t = m1;
+        m1 = m2;
+        m2 = t;
+    }
+    for (int k = 2; k < n_classes; ++k) {
+        if (ph[k] < m1) {
+            m2 = m1;
+            m1 = ph[k];
+        } else if (ph[k] < m2)
+            m2 = ph[k];
+    }
+    g.ph = ph;
+    g.gq = m2 - m1;
+    if (!(g.gq < 2147483647.0)) return false;
+    const int na = (int)((recflags >> 1) & 0x7Fu);
+    int n_pl = (na + 1) * na / 2;
+    if (n_pl > n_classes) n_pl = n_classes;
+    if (n_pl < 1) n_pl = 1;
+    g.n_pl = n_pl;
+    int best = 0, bv = (int)ph[0];
+    for (int k = 1; k < n_pl; ++k)
+        if ((int)ph[k] < bv) {
+            bv = (int)ph[k];
+            best = k;
+        }
+    int count = 0, n_alleles = 0;  // gt_from_pl_idx: triangular index -> (a, b), a <= b
+    while (count < best + 1) {
+        count += n_alleles;
+        ++n_alleles;
+    }
+    g.b = n_alleles - 2;
+    g.a = best - (count - n_alleles) - 1;
+    return true;
+}
+
+// the new value of GQ (which = 0), PL (1) or GT (2)
+__device__ uint32_t fio_geno_value(uint8_t* out, uint32_t n, const FioGeno& g, int which, uint8_t sep) {
+    if (which == 0) return fio_put_int(out, n, (int)g.gq);
+    if (which == 1) {
+        for (int k = 0; k < g.n_pl; ++k) {
+            if (k) n = fio_putc(out, n, ',');
+            n = fio_put_int(out, n, (int)g.ph[k]);
+        }
+        return n;
+    }
+    n = fio_put_int(out, n, g.a);
+    n = fio_putc(out, n, sep);
+    return fio_put_int(out, n, g.b);
+}
+
+// FORMAT and the first sample of a recalibrated record, `fmt` = the bytes after INFO's tab (len of them): the first GQ /
+// PL / GT key of FORMAT gets the new value, keys FORMAT lacks are appended in that order, the sample's values are
+// padded with "." to the keys (and cut to them), FORMAT "." counts as no keys; GT's separator is '|' when a GT value
+// of the input holds one.  Returns the bytes of "FORMAT\tSAMPLE1"; *s1e = where the first sample ends in fmt (the
+// other samples follow untouched).  Streams over the columns: no bound on the keys or the sample's length.
+__device__ uint32_t fio_sample(const uint8_t* fmt, uint32_t len, const FioGeno& g, uint8_t* out, uint32_t* s1e_out) {
+    uint32_t ftab = 0;
+    while (ftab < len && fmt[ftab] != '\t') ++ftab;
+    const uint32_t s1 = ftab < len ? ftab + 1 : len;
+    uint32_t s1e = s1;
+    while (s1e < len && fmt[s1e] != '\t') ++s1e;
+    *s1e_out = s1e;
+    const bool dot = ftab == 1 && fmt[0] == '.';
+    int f_gq = -1, f_pl = -1, f_gt = -1;  // index of the first GQ / PL / GT key
+    uint8_t sep = '/';
+    int nkeys = 0;
+    if (!dot) {  // the keys and the first sample's values side by side: value k of [vs, ve), or none left
+        uint32_t ks = 0, vs = s1;
+        bool vlive = true;
+        for (uint32_t e = 0; e <= ftab; ++e) {
+            if (e < ftab && fmt[e] != ':') continue;
+            uint32_t ve = vs;
+            if (vlive)
+                while (ve < s1e && fmt[ve] != ':') ++ve;
+            if (e - ks == 2) {
+                const uint8_t c0 = fmt[ks], c1 = fmt[ks + 1];
+                const int w = (c0 == 'G' && c1 == 'Q') ? 0 : (c0 == 'P' && c1 == 'L') ? 1 : (c0 == 'G' && c1 == 'T') ? 2 : -1;
+                if (w == 0 && f_gq < 0) f_gq = nkeys;
+                if (w == 1 && f_pl < 0) f_pl = nkeys;
+                if (w == 2 && f_gt < 0) f_gt = nkeys;
+                if (w == 2 && vlive)
+                    for (uint32_t u = vs; u < ve; ++u)
+                        if (fmt[u] == '|') sep = '|';
+            }
+            ++nkeys;
+            if (vlive) {
+                if (ve < s1e) vs = ve + 1;
+                else vlive = false;
+            }
+            ks = e + 1;
+        }
+    }
+    const uint8_t* K = reinterpret_cast<const uint8_t*>("GQPLGT");
+    uint32_t n = dot ? 0u : fio_put(out, 0, fmt, ftab);
+    int cnt = nkeys;
+    for (int w = 0; w < 3; ++w)
+        if ((w == 0 ? f_gq : w == 1 ? f_pl : f_gt) < 0) {
+            if (cnt++) n = fio_putc(out, n, ':');
+            n = fio_put(out, n, K + 2 * w, 2);
+        }
+    n = fio_putc(out, n, '\t');
+    uint32_t vs = s1;
+    bool vlive = true;
+    for (int k = 0; k < nkeys; ++k) {
+        uint32_t ve = vs;
+        if (vlive)
+            while (ve < s1e && fmt[ve] != ':') ++ve;
+        if (k) n = fio_putc(out, n, ':');
+        const int w = k == f_gq ? 0 : k == f_pl ? 1 : k == f_gt ? 2 : -1;
+        if (w >= 0) n = fio_geno_value(out, n, g, w, sep);
+        else if (vlive) n = fio_put(out, n, fmt + vs, ve - vs);
+        else n = fio_putc(out, n, '.');
+        if (vlive) {
+            if (ve < s1e) vs = ve + 1;
+            else vlive = false;
+        }
+    }
+    cnt = nkeys;
+    for (int w = 0; w < 3; ++w)
+        if ((w == 0 ? f_gq : w == 1 ? f_pl : f_gt) < 0) {
+            if (cnt++) n = fio_putc(out, n, ':');
+            n = fio_geno_value(out, n, g, w, sep);
+        }
+    return n;
+}
+
+// splice_len: the length of every edited line (and what splice_copy needs of it: the formatted score, the annotation bits);
+// a record the rules here do not cover raises `fallback` and the caller hands the range to the host writer
 __global__ void __launch_bounds__(256) splice_len(const uint8_t* __restrict__ text, const int64_t* __restrict__ line_start,
                                                   const ugvc_recinfo* __restrict__ recinfo, const uint8_t* __restrict__ low_score,
-                                                  const double* __restrict__ qual, int64_t n, int flags,
+                                                  const double* __restrict__ qual, int64_t n, const FioEdits ed,
                                                   int64_t* __restrict__ out_len, uint8_t* __restrict__ score_txt, int* fallback) {
+    const bool recal = ed.phreds != nullptr;
+    const bool owq = ed.with_model && (ed.flags & UGVC_FILE_OVERWRITE_QUAL);
+    const bool want_num = ed.with_model && (!recal || owq);  // TREE_SCORE, or QUAL = GQ
+    unsigned long long n_bl = 0;
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
         const FioRec r = fio_rec(line_start, recinfo, i);
+        const ugvc_recinfo ri = recinfo[i];
+        FioGeno g;
+        bool ok = r.ok && (!recal || fio_geno(ed.phreds + (size_t)i * ed.n_classes, ed.n_classes, ri.flags, g));
         char num[16];
-        const int sl = fio_format_g((float)qual[i], num);
-        if (!r.ok || sl == 0) {
+        int sl = 0;
+        if (ok && want_num) {
+            sl = fio_format_g((float)(recal ? g.gq : qual[i]), num);
+            ok = sl != 0;
+        }
+        if (!ok) {
             atomicExch(fallback, 1);
             out_len[i] = 0;
             continue;
@@ -177,17 +394,29 @@ __global__ void __launch_bounds__(256) splice_len(const uint8_t* __restrict__ te
         uint8_t* st = score_txt + (size_t)i * 16;
         st[15] = (uint8_t)sl;
         for (int c = 0; c < sl; ++c) st[c] = (uint8_t)num[c];
+        const uint32_t mask = fio_bl_mask(ri.pos, (ed.flags & UGVC_FILE_BLACKLIST_CG) && (ri.flags & 1u), ed.n_bl, ed.bl_pos, ed.bl_pos_off);
+        ed.bl_mask[i] = mask;
+        n_bl += mask != 0u;
         const uint8_t* line = text + line_start[i];
-        const bool low = low_score[i] != 0;
+        const bool low = ed.with_model && low_score[i] != 0;
         const uint32_t il = r.x0 - 1u - r.i0;
-        uint32_t total = r.q0;                                                                 // columns 1-5 with their tabs
-        total += ((flags & UGVC_FILE_OVERWRITE_QUAL) ? (uint32_t)sl : r.f0 - 1u - r.q0) + 1u;  // QUAL, tab
-        total += fio_filter(line + r.f0, r.i0 - 1u - r.f0, low, nullptr) + 1u;                 // FILTER, tab
-        total += il + FIO_SCORE_KEY_LEN + (uint32_t)sl;                                         // INFO;TREE_SCORE=<score>
-        if ((flags & UGVC_FILE_BLACKLIST_CG) && (recinfo[i].flags & 1u)) total += FIO_CG_LEN;
-        if (r.x0 <= r.len) total += 1u + (r.len - r.x0);                                        // tab, FORMAT and samples
-        out_len[i] = (int64_t)total + 1;                                                        // newline
+        uint32_t total = r.q0;                                                    // columns 1-5 with their tabs
+        total += (owq ? (uint32_t)sl : r.f0 - 1u - r.q0) + 1u;                    // QUAL, tab
+        total += fio_filter(line + r.f0, r.i0 - 1u - r.f0, low, nullptr) + 1u;    // FILTER, tab
+        total += il;                                                              // INFO
+        if (ed.with_model && !recal) total += FIO_SCORE_KEY_LEN + (uint32_t)sl;   // ;TREE_SCORE=<score>
+        if (mask) total += fio_blacklst(mask, ed.n_bl, ed.bl_name, ed.bl_name_off, nullptr);  // ;BLACKLST=<annotations>
+        if (r.x0 <= r.len) {                                                      // tab, FORMAT and samples
+            total += 1u + (r.len - r.x0);
+            if (recal) {
+                uint32_t s1e = 0;
+                const uint32_t sn = fio_sample(line + r.x0, r.len - r.x0, g, nullptr, &s1e);
+                total = total - s1e + sn;
+            }
+        }
+        out_len[i] = (int64_t)total + 1;  // newline
     }
+    if (n_bl) atomicAdd(ed.n_blacklisted, n_bl);
 }
 
 __device__ __forceinline__ void fio_copy(uint8_t* dst, const uint8_t* src, uint32_t n, unsigned lane) {
@@ -196,10 +425,13 @@ __device__ __forceinline__ void fio_copy(uint8_t* dst, const uint8_t* src, uint3
 
 __global__ void __launch_bounds__(256) splice_copy(const uint8_t* __restrict__ text, const int64_t* __restrict__ line_start,
                                                    const ugvc_recinfo* __restrict__ recinfo, const uint8_t* __restrict__ low_score,
-                                                   int64_t n, int flags, const int64_t* __restrict__ out_start,
+                                                   int64_t n, const FioEdits ed, const int64_t* __restrict__ out_start,
                                                    const uint8_t* __restrict__ score_txt, uint8_t* __restrict__ out, int* fallback) {
+    const unsigned FULL = 0xffffffffu;
     const unsigned lane = threadIdx.x & 31u;
     const int64_t warp0 = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5, n_warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    const bool recal = ed.phreds != nullptr;
+    const bool owq = ed.with_model && (ed.flags & UGVC_FILE_OVERWRITE_QUAL);
     for (int64_t i = warp0; i < n; i += n_warps) {
         const FioRec r = fio_rec(line_start, recinfo, i);
         if (!r.ok) continue;
@@ -209,7 +441,7 @@ __global__ void __launch_bounds__(256) splice_copy(const uint8_t* __restrict__ t
         uint8_t* o = out + out_start[i];
         fio_copy(o, line, r.q0, lane);
         o += r.q0;
-        if (flags & UGVC_FILE_OVERWRITE_QUAL) {
+        if (owq) {
             fio_copy(o, st, sl, lane);
             o += sl;
         } else {
@@ -220,15 +452,18 @@ __global__ void __launch_bounds__(256) splice_copy(const uint8_t* __restrict__ t
         uint32_t fn = 0;
         if (lane == 0) {
             o[0] = '\t';
-            fn = fio_filter(line + r.f0, r.i0 - 1u - r.f0, low_score[i] != 0, o + 1);
+            fn = fio_filter(line + r.f0, r.i0 - 1u - r.f0, ed.with_model && low_score[i] != 0, o + 1);
             o[1 + fn] = '\t';
         }
-        fn = __shfl_sync(0xffffffffu, fn, 0);
+        fn = __shfl_sync(FULL, fn, 0);
         o += fn + 2u;
-        // INFO: copied as it is when it is "plain" (hostio.cpp: no empty piece, not ".", neither key already there)
+        // INFO: copied as it is when it is "plain" (hostio.cpp: no empty piece, not ".", neither key already there).
+        // Under out_end each lane also notes the first piece it sees that starts with "END=" (ugvc_info_end: the first
+        // such piece of the column decides)
         const uint8_t* ip = line + r.i0;
         const uint32_t il = r.x0 - 1u - r.i0;
         bool odd = il == 0 || (il == 1 && ip[0] == '.') || ip[0] == ';' || ip[il - 1] == ';';
+        uint32_t endk = 0xFFFFFFFFu;
         for (uint32_t k = lane; k < il; k += 32u) {
             const uint8_t c = ip[k];
             o[k] = c;
@@ -245,23 +480,61 @@ __global__ void __launch_bounds__(256) splice_copy(const uint8_t* __restrict__ t
                 for (int z = 1; z < 9 && eq; ++z) eq = ip[k + z] == (uint8_t)key[z];
                 odd |= eq;
             }
+            if (c == 'E' && endk == 0xFFFFFFFFu && k + 4 <= il && (k == 0 || ip[k - 1] == ';') && ip[k + 1] == 'N' &&
+                ip[k + 2] == 'D' && ip[k + 3] == '=')
+                endk = k;
         }
-        if (__any_sync(0xffffffffu, odd)) {
+        if (__any_sync(FULL, odd)) {
             if (lane == 0) atomicExch(fallback, 1);
         }
+        if (ed.out_end) {
+            endk = __reduce_min_sync(FULL, endk);
+            if (lane == 0) {
+                // ugvc_info_end: a piece "END=" + 1..10 digits gives the value, any other END= piece gives none
+                int64_t v = 0;
+                if (endk != 0xFFFFFFFFu) {
+                    uint32_t q = endk + 4u;
+                    while (q < il && ip[q] != ';') ++q;
+                    const uint32_t pl = q - endk;
+                    bool digits = pl > 4u && pl <= 14u;
+                    for (uint32_t d = endk + 4u; d < q && digits; ++d) {
+                        digits = ip[d] >= '0' && ip[d] <= '9';
+                        v = v * 10 + (ip[d] - '0');
+                    }
+                    if (!digits) v = 0;
+                }
+                ed.out_end[i] = v;
+            }
+        }
         o += il;
-        if (lane < FIO_SCORE_KEY_LEN) o[lane] = (uint8_t)FIO_SCORE_KEY[lane];
-        o += FIO_SCORE_KEY_LEN;
-        fio_copy(o, st, sl, lane);
-        o += sl;
-        if ((flags & UGVC_FILE_BLACKLIST_CG) && (recinfo[i].flags & 1u)) {
-            if (lane < FIO_CG_LEN) o[lane] = (uint8_t)FIO_CG_TEXT[lane];
-            o += FIO_CG_LEN;
+        if (ed.with_model && !recal) {
+            if (lane < FIO_SCORE_KEY_LEN) o[lane] = (uint8_t)FIO_SCORE_KEY[lane];
+            o += FIO_SCORE_KEY_LEN;
+            fio_copy(o, st, sl, lane);
+            o += sl;
+        }
+        const uint32_t mask = ed.bl_mask[i];
+        if (mask) {
+            uint32_t bn = 0;
+            if (lane == 0) bn = fio_blacklst(mask, ed.n_bl, ed.bl_name, ed.bl_name_off, o);
+            o += __shfl_sync(FULL, bn, 0);
         }
         if (r.x0 <= r.len) {
             if (lane == 0) o[0] = '\t';
-            fio_copy(o + 1, line + r.x0, r.len - r.x0, lane);
-            o += 1u + (r.len - r.x0);
+            ++o;
+            uint32_t from = 0;  // FORMAT and the samples from here on are copied as they are
+            if (recal) {
+                uint32_t sn = 0, s1e = 0;
+                if (lane == 0) {
+                    FioGeno g;
+                    fio_geno(ed.phreds + (size_t)i * ed.n_classes, ed.n_classes, recinfo[i].flags, g);  // true: splice_len
+                    sn = fio_sample(line + r.x0, r.len - r.x0, g, o, &s1e);
+                }
+                o += __shfl_sync(FULL, sn, 0);
+                from = __shfl_sync(FULL, s1e, 0);
+            }
+            fio_copy(o, line + r.x0 + from, r.len - r.x0 - from, lane);
+            o += r.len - r.x0 - from;
         }
         if (lane == 0) o[0] = '\n';
     }
@@ -474,20 +747,20 @@ cudaError_t fio_scan_u64(void* tmp, size_t& tmp_bytes, const uint64_t* in, uint6
     return cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, in, out, n, st);
 }
 void fio_launch_splice_len(const uint8_t* text, const int64_t* line_start, const ugvc_recinfo* recinfo, const uint8_t* low,
-                           const double* qual, int64_t n, int flags, int64_t* out_len, uint8_t* score_txt, int* fallback,
-                           int sm_count, cudaStream_t st) {
+                           const double* qual, int64_t n, const FioEdits& ed, int64_t* out_len, uint8_t* score_txt,
+                           int* fallback, int sm_count, cudaStream_t st) {
     if (n <= 0) return;
     int64_t blocks = (n + 255) / 256;
     if (blocks > (int64_t)sm_count * 16) blocks = (int64_t)sm_count * 16;
-    splice_len<<<(unsigned)blocks, 256, 0, st>>>(text, line_start, recinfo, low, qual, n, flags, out_len, score_txt, fallback);
+    splice_len<<<(unsigned)blocks, 256, 0, st>>>(text, line_start, recinfo, low, qual, n, ed, out_len, score_txt, fallback);
 }
 void fio_launch_splice_copy(const uint8_t* text, const int64_t* line_start, const ugvc_recinfo* recinfo, const uint8_t* low,
-                            int64_t n, int flags, const int64_t* out_start, const uint8_t* score_txt, uint8_t* out,
+                            int64_t n, const FioEdits& ed, const int64_t* out_start, const uint8_t* score_txt, uint8_t* out,
                             int* fallback, int sm_count, cudaStream_t st) {
     if (n <= 0) return;
     int64_t blocks = (n + 7) / 8;
     if (blocks > (int64_t)sm_count * 32) blocks = (int64_t)sm_count * 32;
-    splice_copy<<<(unsigned)blocks, 256, 0, st>>>(text, line_start, recinfo, low, n, flags, out_start, score_txt, out, fallback);
+    splice_copy<<<(unsigned)blocks, 256, 0, st>>>(text, line_start, recinfo, low, n, ed, out_start, score_txt, out, fallback);
 }
 cudaError_t fio_launch_deflate(const uint8_t* text, size_t n_bytes, const DefTables* tables, uint8_t* blocks, uint32_t* bsize,
                                int n_blocks, int encoder, cudaStream_t st) {

@@ -8,11 +8,28 @@
 struct DefTables;
 cudaError_t fio_scan_i64(void* tmp, size_t& tmp_bytes, const int64_t* in, int64_t* out, int64_t n, cudaStream_t st);
 cudaError_t fio_scan_u64(void* tmp, size_t& tmp_bytes, const uint64_t* in, uint64_t* out, int n, cudaStream_t st);
+
+// What the record writer edits besides FILTER (ugvc_filter_bgzf_edits), all device pointers.  Annotation bit 0 of a
+// record is the CG insertion flag (UGVC_FILE_BLACKLIST_CG), bit k + 1 blacklist k.
+struct FioEdits {
+    int with_model;              // 0: FILTER keeps its pieces, no TREE_SCORE, QUAL untouched
+    int flags;                   // UGVC_FILE_*
+    const double* phreds;        // [n][n_classes]: GT / GQ / PL of the first sample are rewritten (NULL: they are not)
+    int n_classes;
+    int n_bl;                    // blacklists, <= UGVC_MAX_BLACKLISTS
+    const int64_t* bl_pos;       // sorted POS of each blacklist, concatenated; blacklist k at [bl_pos_off[k], bl_pos_off[k + 1])
+    const int64_t* bl_pos_off;
+    const uint8_t* bl_name;      // the value text of each blacklist (',' joined pieces, maybe empty) at [bl_name_off[k], ..[k + 1])
+    const int32_t* bl_name_off;
+    uint32_t* bl_mask;           // [n] scratch: the annotation bits of each record (splice_len -> splice_copy)
+    unsigned long long* n_blacklisted;  // += records with at least one annotation bit
+    int64_t* out_end;            // [n] INFO/END of each record, 0 where none (ugvc_info_end's rule); NULL: not wanted
+};
 void fio_launch_splice_len(const uint8_t* text, const int64_t* line_start, const ugvc_recinfo* recinfo, const uint8_t* low,
-                           const double* qual, int64_t n, int flags, int64_t* out_len, uint8_t* score_txt, int* fallback,
-                           int sm_count, cudaStream_t st);
+                           const double* qual, int64_t n, const FioEdits& ed, int64_t* out_len, uint8_t* score_txt,
+                           int* fallback, int sm_count, cudaStream_t st);
 void fio_launch_splice_copy(const uint8_t* text, const int64_t* line_start, const ugvc_recinfo* recinfo, const uint8_t* low,
-                            int64_t n, int flags, const int64_t* out_start, const uint8_t* score_txt, uint8_t* out,
+                            int64_t n, const FioEdits& ed, const int64_t* out_start, const uint8_t* score_txt, uint8_t* out,
                             int* fallback, int sm_count, cudaStream_t st);
 // encoder: FIO_ENC_WARP (fio_deflate_warp, the default) or FIO_ENC_THREAD (fio_deflate, one thread per block)
 #define FIO_ENC_WARP 0

@@ -201,8 +201,11 @@ class _Splicer:
         ri = res["recinfo"]
         beg = ri["pos"].astype(np.int64) - 1
         self._check_writer()
+        end = beg + np.maximum(1, (ri["flags"] >> 8).astype(np.int64))
+        if self.index_info_end:
+            end = np.where(res["end"] > beg, res["end"], end)  # the INFO/END the device writer read; the rule of write_batch
         self._queue.put(((list(contigs), np.asarray(bounds, dtype=np.int64)), (res["bgzf"], res["block_csize"], release), n, beg,
-                         beg + np.maximum(1, (ri["flags"] >> 8).astype(np.int64)), res["line_start"]))
+                         end, res["line_start"]))
 
     def _write_spliced(self, contig, data, n: int, beg: np.ndarray, end: np.ndarray, out_ls: np.ndarray):
         t0 = time.perf_counter()
@@ -554,14 +557,12 @@ def run(argv: list[str]):  # noqa: C901, PLR0912, PLR0915
             logger.info(f"rank {rank}/{world}: {len(contigs)} of {len(all_contigs)} contigs")
 
         # compressed bytes both ways: the contig's BGZF blocks go to the device as they are, come back filtered, edited
-        # and compressed again (ugvc_filter_bgzf); what that path does not cover keeps the host readers / writers
-        # (INFO/END: the host writer ends a record's index interval at END like htslib; the device writer's recinfo does
-        # not carry END, so on that path the interval is POS + len(REF) -- gVCF blocks / symbolic alleles: --host_io)
+        # and compressed again (ugvc_filter_bgzf_edits: with or without a model, blacklists, --recalibrate_genotype; the
+        # writer also reads INFO/END, where the index ends a record when the header declares the tag, as htslib does).
+        # --treat_multiallelics keeps the host readers / writers: its index pass, split build and scored pass over a
+        # whole contig are not chained on the device
         out.index_info_end = "END" in header.info
-        device_io = bool(with_model and not split_sites and not recal and blacklists is None and not args.host_io)
-        if device_io and out.index_info_end:
-            logger.info("the header declares INFO/END: index intervals on the device file path are POS + len(REF); "
-                        "--host_io ends them at END")
+        device_io = bool(not split_sites and not args.host_io)
         file_flags = (lib.FILE_OVERWRITE_QUAL if args.overwrite_qual_tag else 0) | \
                      (lib.FILE_BLACKLIST_CG if args.blacklist_cg_insertions else 0)
 
@@ -694,7 +695,9 @@ def run(argv: list[str]):  # noqa: C901, PLR0912, PLR0915
             groups, cur, cur_bytes = [], [], 0
             for c, vb, ve in pieces:
                 span = (ve >> 16) - (vb >> 16)
-                if cur and (multi or vb != cur[-1][2] or cur_bytes + span > group_bytes + group_bytes // 4):
+                # blacklist positions are uploaded per call for one contig: with blacklists a group holds one contig
+                if cur and (multi or vb != cur[-1][2] or cur_bytes + span > group_bytes + group_bytes // 4 or
+                            (blacklists is not None and c != cur[-1][0])):
                     groups.append(cur)
                     cur, cur_bytes = [], 0
                 cur.append((c, vb, ve))
@@ -743,17 +746,19 @@ def run(argv: list[str]):  # noqa: C901, PLR0912, PLR0915
         flying: list[tuple] = []
         n_calls = 0
 
-        def device_call(lane: int, comp, skip: int, take: int, in_bufs: dict, starts):
+        def device_call(lane: int, comp, skip: int, take: int, in_bufs: dict, starts, bl_pos):
             ctx.bind_thread()
             n_max = take // 32 + 1024
             # VCF text deflates to well under half its size; text that does not comes back as UGVC_E_FALLBACK
-            out_bufs = out_pool.acquire({"out": (take * 5 // 8 + (1 << 20), np.uint8),
-                                         "blocks": ((take + n_max * 64) // lib.DEF_CHUNK + 16, np.uint32),
-                                         "ri": (n_max, lib.RECINFO_DTYPE), "ls": (n_max + 1, np.int64), "low": (n_max, np.uint8)},
-                                        grow=max_span / max(1, comp.size))
+            sizes = {"out": (take * 5 // 8 + (1 << 20), np.uint8), "blocks": ((take + n_max * 64) // lib.DEF_CHUNK + 16, np.uint32),
+                     "ri": (n_max, lib.RECINFO_DTYPE), "ls": (n_max + 1, np.int64), "low": (n_max, np.uint8)}
+            if out.index_info_end:
+                sizes["end"] = (n_max, np.int64)
+            out_bufs = out_pool.acquire(sizes, grow=max_span / max(1, comp.size))
             try:
-                res = ctx.filter_bgzf(comp, skip, take, args.decision_threshold, file_flags, n_max, lane=lane,
-                                      bufs={k: v[1] for k, v in out_bufs.items()})
+                res = ctx.filter_bgzf_edits(comp, skip, take, args.decision_threshold, file_flags, n_max, with_model=with_model,
+                                            recalibrate_genotype=recal, blacklists=bl_pos, want_end=out.index_info_end,
+                                            lane=lane, bufs={k: v[1] for k, v in out_bufs.items()})
                 first = ctx.filter_bgzf_first_records(starts, lane=lane) if res is not None else None
                 ms = ctx.filter_bgzf_stage_ms(lane) if res is not None else None
             except BaseException:
@@ -789,15 +794,16 @@ def run(argv: list[str]):  # noqa: C901, PLR0912, PLR0915
                 logger.info("Writing records")
                 out.write_device_batch([g[0] for g in live], bounds, res, release=lambda b=out_bufs: out_pool.release(b))
                 totals["n_records"] += res["n_records"]
-                totals["n_low_score"] += int(res["low_score"].sum())
-                if args.blacklist_cg_insertions:
-                    n_cg = int(np.count_nonzero(res["recinfo"]["flags"] & 1))
-                    totals["n_cg"] += n_cg
-                    totals["n_blacklisted"] += n_cg
+                if with_model:
+                    totals["n_low_score"] += int(res["low_score"].sum())
+                if with_bl:  # what blacklist_codes counts on the host path
+                    totals["n_cg"] += int(np.count_nonzero(res["recinfo"]["flags"] & 1))
+                    totals["n_blacklisted"] += res["n_blacklisted"]
                 for c in dict.fromkeys(g[0] for g in live):
                     logger.info(f"{c} done")
 
         prefetch = ThreadPoolExecutor(max_workers=1, thread_name_prefix="ugvc-bgzf-reader")
+        bl_last = [None, None]  # (contig, its blacklist positions) of the last device group
         pending = prefetch.submit(load_work, work[0]) if work else None
         for gi, group in enumerate(work):
             for c in dict.fromkeys(g[0] for g in group):
@@ -814,9 +820,16 @@ def run(argv: list[str]):  # noqa: C901, PLR0912, PLR0915
                 host_contig(group[0][0], loaded)
                 continue
             _tag, comp, skip, take, in_bufs, live, starts = loaded  # ("device", compressed blocks, ...)
+            if blacklists is not None:
+                logger.info("Applying blacklist")
             if args.blacklist_cg_insertions:
                 logger.info("Marking CG insertions")
-            if not key_order_set:
+            bl_pos = None
+            if blacklists is not None:  # (one contig a group) a long contig is many groups: its positions are kept
+                if bl_last[0] != live[0][0]:
+                    bl_last[:] = [live[0][0], _blacklist_positions(blacklists, live[0][0])]
+                bl_pos = bl_last[1]
+            if not key_order_set and with_model:
                 head = bgzf_io.first_block_text(comp, skip)
                 ctx.set_key_order(*lib.learn_key_order(head[: head.rfind(b"\n") + 1]))
                 key_order_set = True
@@ -829,7 +842,7 @@ def run(argv: list[str]):  # noqa: C901, PLR0912, PLR0915
                 ctx.reserve(reserved[0], reserved[1], n_lanes)
             seconds["alloc"] += time.perf_counter() - t_alloc
             drain_device(n_lanes - 1)  # at most n_lanes calls in flight, each on its own lane and stream
-            flying.append((live, gpu_pool.submit(device_call, n_calls % n_lanes, comp, skip, take, in_bufs, starts)))
+            flying.append((live, gpu_pool.submit(device_call, n_calls % n_lanes, comp, skip, take, in_bufs, starts, bl_pos)))
             n_calls += 1
             if n_calls == 1:
                 drain_device(0)  # the first call alone: every lazy one-time set-up of the path happens on one thread

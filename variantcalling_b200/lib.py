@@ -35,6 +35,13 @@ RECINFO_DTYPE = np.dtype([("pos", "<i4"), ("qual_off", "<u2"), ("filter_off", "<
                           ("format_off", "<u2"), ("flags", "<u4")])
 
 
+class FileEdits(C.Structure):
+    """ugvc_file_edits (include/ugvc_b200.h)."""
+    _fields_ = [("with_model", C.c_int), ("recalibrate_genotype", C.c_int), ("n_blacklists", C.c_int),
+                ("blacklist_pos", C.c_void_p), ("blacklist_pos_off", C.c_void_p), ("blacklist_names", C.c_void_p),
+                ("blacklist_name_off", C.c_void_p), ("out_end", C.c_void_p), ("n_blacklisted", C.c_int64)]
+
+
 class Counts(C.Structure):
     _fields_ = [("n_records", C.c_int64), ("n_low_score", C.c_int64), ("n_pass", C.c_int64), ("n_cg", C.c_int64)]
 
@@ -119,6 +126,11 @@ SIGNATURES = {
                                        C.POINTER(C.c_uint32), C.POINTER(C.c_uint64)]),
     "ugvc_filter_bgzf": (C.c_int, [_vp, C.c_int, _vp, _sz, C.c_uint32, C.c_uint64, C.c_double, C.c_int, _vp, _sz, C.POINTER(_sz),
                                    _vp, _sz, C.POINTER(_sz), _vp, _vp, _vp, _sz, C.POINTER(C.c_int64)]),
+    "ugvc_filter_bgzf_edits": (C.c_int, [_vp, C.c_int, _vp, _sz, C.c_uint32, C.c_uint64, C.c_double, C.c_int, C.POINTER(FileEdits),
+                                         _vp, _sz, C.POINTER(_sz), _vp, _sz, C.POINTER(_sz), _vp, _vp, _vp, _sz,
+                                         C.POINTER(C.c_int64)]),
+    "ugvc_test_write_records": (C.c_int64, [_vp, _vp, _sz, _vp, _vp, C.c_int64, _vp, _vp, _vp, C.c_int, C.c_int,
+                                            C.POINTER(FileEdits), _vp, _sz, _vp]),
     "ugvc_filter_bgzf_stage_ms": (C.c_int, [_vp, C.c_int, _vp]),
     "ugvc_filter_bgzf_first_records": (C.c_int, [_vp, C.c_int, _vp, C.c_int, _vp]),
     "ugvc_test_parse_float": (C.c_int, [C.c_char_p, C.POINTER(C.c_float), C.POINTER(C.c_double),
@@ -183,6 +195,21 @@ class PinnedBuffer:
             self.free()
         except Exception:  # noqa: BLE001, S110
             pass
+
+
+def _file_edits(with_model: bool, recalibrate: bool, blacklists, end: np.ndarray | None):
+    """A FileEdits struct and the arrays it points into (kept alive by the caller)."""
+    bl = blacklists or []
+    names = [a.encode() if isinstance(a, str) else bytes(a) for a, _ in bl]
+    pos = [np.ascontiguousarray(p, dtype=np.int64) for _, p in bl]
+    pos_all = np.concatenate(pos) if pos else np.zeros(0, np.int64)
+    pos_off = np.concatenate(([0], np.cumsum([p.size for p in pos]))).astype(np.int64)
+    name_buf = np.frombuffer(b"".join(names) or b"\0", dtype=np.uint8)
+    name_off = np.concatenate(([0], np.cumsum([len(a) for a in names]))).astype(np.int64)
+    e = FileEdits(int(bool(with_model)), int(bool(recalibrate)), len(bl), pos_all.ctypes.data if pos_all.size else None,
+                  pos_off.ctypes.data, name_buf.ctypes.data, name_off.ctypes.data,
+                  end.ctypes.data if end is not None else None, 0)
+    return e, (pos_all, pos_off, name_buf, name_off)
 
 
 class Context:
@@ -324,6 +351,56 @@ class Context:
                     lane: int = 0, bufs: dict | None = None) -> dict | None:
         """One range of whole lines: compressed blocks in, filtered + scored + edited records out as BGZF blocks
         (see ugvc_filter_bgzf).  Returns None when the range needs the general host writer."""
+        return self._filter_bgzf(bgzf, skip_head, take_bytes, threshold, flags, max_records, lane, bufs, None)
+
+    def filter_bgzf_edits(self, bgzf: np.ndarray, skip_head: int, take_bytes: int, threshold: float, flags: int,
+                          max_records: int, *, with_model: bool = True, recalibrate_genotype: bool = False,
+                          blacklists: list[tuple[str, np.ndarray]] | None = None, want_end: bool = False, lane: int = 0,
+                          bufs: dict | None = None) -> dict | None:
+        """:meth:`filter_bgzf` with the rest of the record edits (see ugvc_filter_bgzf_edits): a model-less plan
+        (with_model=False), --recalibrate_genotype (needs enable_phreds(1) before reserve), blacklists as
+        [(annotation, sorted POS of the range's contig)], and with want_end the INFO/END of every record ("end", 0 where
+        there is none).  The result also holds "n_blacklisted".  None when the range needs the general host writer."""
+        end = None
+        if want_end:
+            end = bufs["end"] if bufs is not None and "end" in bufs else np.empty(max(1, max_records), np.int64)
+        e, keep = _file_edits(with_model, recalibrate_genotype, blacklists, end)
+        res = self._filter_bgzf(bgzf, skip_head, take_bytes, threshold, flags, max_records, lane, bufs, e)
+        if res is not None:
+            res["n_blacklisted"] = int(e.n_blacklisted)
+            if end is not None:
+                res["end"] = end[: res["n_records"]]
+        return res
+
+    def test_write_records(self, text, line_start, recinfo, flags: int, *, low_score=None, qual=None, phreds=None,
+                           with_model: bool = True, recalibrate_genotype: bool = False, blacklists=None,
+                           want_end: bool = False) -> dict | None:
+        """The device record writer alone on caller records (ugvc_test_write_records): {"text", "line_start",
+        "n_blacklisted"[, "end"]}, or None when it hands the records back."""
+        buf = np.frombuffer(text, dtype=np.uint8) if isinstance(text, (bytes, bytearray)) else np.ascontiguousarray(text)
+        ls = np.ascontiguousarray(line_start, dtype=np.int64)
+        ri = np.ascontiguousarray(recinfo)
+        n = ls.size - 1
+        end = np.zeros(max(1, n), np.int64) if want_end else None
+        e, keep = _file_edits(with_model, recalibrate_genotype, blacklists, end)  # noqa: F841  (keep: alive for the call)
+        ph = None if phreds is None else np.ascontiguousarray(phreds, dtype=np.float64)
+        low = None if low_score is None else np.ascontiguousarray(low_score, dtype=np.uint8)
+        q = None if qual is None else np.ascontiguousarray(qual, dtype=np.float64)
+        out = np.empty(buf.size + n * 256 + 4096, dtype=np.uint8)
+        out_ls = np.empty(n + 1, dtype=np.int64)
+        nb = self.lib.ugvc_test_write_records(self.h, _ptr(buf), buf.size, _ptr(ls), _ptr(ri), n, _ptr(low), _ptr(q), _ptr(ph),
+                                              0 if ph is None else (ph.shape[1] if ph.ndim == 2 else 0), flags, C.byref(e),
+                                              _ptr(out), out.size, _ptr(out_ls))
+        if nb == UGVC_E_FALLBACK:
+            return None
+        if nb < 0:
+            self._check(int(nb))
+        res = {"text": out[:nb].tobytes(), "line_start": out_ls, "n_blacklisted": int(e.n_blacklisted)}
+        if end is not None:
+            res["end"] = end[:n]
+        return res
+
+    def _filter_bgzf(self, bgzf, skip_head, take_bytes, threshold, flags, max_records, lane, bufs, edits):
         comp = np.ascontiguousarray(bgzf, dtype=np.uint8)
         if bufs is not None:  # the caller's (pinned, reused) buffers: out, blocks, ri, ls, low
             out, blocks, ri, ls, low = bufs["out"], bufs["blocks"], bufs["ri"], bufs["ls"], bufs["low"]
@@ -335,9 +412,13 @@ class Context:
             ls = np.empty(max_records + 1, dtype=np.int64)
             low = np.empty(max_records, dtype=np.uint8)
         nb, nblk, n = C.c_size_t(), C.c_size_t(), C.c_int64()
-        rc = self.lib.ugvc_filter_bgzf(self.h, lane, _ptr(comp), comp.size, skip_head, take_bytes, threshold, flags, _ptr(out),
-                                       out.size, C.byref(nb), _ptr(blocks), blocks.size, C.byref(nblk), _ptr(ri), _ptr(ls),
-                                       _ptr(low), max_records, C.byref(n))
+        args = (_ptr(out), out.size, C.byref(nb), _ptr(blocks), blocks.size, C.byref(nblk), _ptr(ri), _ptr(ls), _ptr(low),
+                max_records, C.byref(n))
+        if edits is None:
+            rc = self.lib.ugvc_filter_bgzf(self.h, lane, _ptr(comp), comp.size, skip_head, take_bytes, threshold, flags, *args)
+        else:
+            rc = self.lib.ugvc_filter_bgzf_edits(self.h, lane, _ptr(comp), comp.size, skip_head, take_bytes, threshold, flags,
+                                                 C.byref(edits), *args)
         if rc == UGVC_E_FALLBACK:
             return None
         self._check(rc)
