@@ -297,8 +297,8 @@ int ugvc_filter_bgzf(ugvc_ctx* ctx, int lane, const uint8_t* bgzf, size_t n_byte
                      double threshold, int flags, uint8_t* out_bgzf, size_t out_capacity, size_t* out_bytes,
                      uint32_t* out_block_csize, size_t block_capacity, size_t* out_n_blocks, ugvc_recinfo* out_recinfo,
                      int64_t* out_line_start, uint8_t* out_low_score, size_t capacity_records, int64_t* out_n_records);
-/* ugvc_filter_bgzf with the rest of the tool's record edits, so that every run but --treat_multiallelics can stay on
- * the device (ugvc_filter_bgzf is this call with with_model = 1 and everything else zero):
+/* ugvc_filter_bgzf with the rest of the tool's record edits (ugvc_filter_bgzf is this call with with_model = 1 and
+ * everything else zero; --treat_multiallelics runs through ugvc_filter_bgzf_split, which writes the same way):
  *   with_model = 0     a model-less plan (FILTER keeps its non-empty pieces, PASS when none is left; no TREE_SCORE;
  *                      QUAL untouched; out_low_score all 0)
  *   recalibrate_genotype  --recalibrate_genotype (filter_variants_pipeline.py:203-215): GQ = int(second smallest -
@@ -426,6 +426,35 @@ int ugvc_ma_data_error(const ugvc_ma* h, int64_t* group, int32_t* code);
 int ugvc_ma_fetch(ugvc_ma* h, uint8_t* out_text, size_t capacity, int32_t* out_origin, uint8_t* out_n_rows,
                   uint8_t* out_n_alleles, size_t capacity_groups);
 int ugvc_ma_merge(ugvc_ma* h, const double* lik, int64_t n_rows, int n_classes, double* out, int width);
+/* --treat_multiallelics on the file path: ugvc_filter_bgzf_edits for one whole contig a call (overlap clusters must not
+ * be cut), with the split branch between the inflate and the record writer, every stage on `lane`'s stream and device
+ * pointers: the blocks are inflated (skip_head / take_bytes as for ugvc_filter_bgzf), indexed by K1 of the model-less
+ * plan of `index_ctx` (its lane `lane` keeps the line starts / recinfo), split by `ma` (ugvc_ma_build on the device text,
+ * ref_seq = the contig's reference sequence, host memory), the scored pass (K1..K3 of ctx, fp64 likelihoods) runs on
+ * the split text, ugvc_ma_merge folds the likelihoods into N x W (W = max(n_classes, widest group)), and the score
+ * math of filter_variants_pipeline.py:174-180,192 runs on the device (phreds = -10 log10(lik + 1e-10) over all W
+ * columns, qual = max(30 + ph0 - min(ph[1:]), 0), LOW_SCORE = qual <= threshold; exactly 100 where lik + 1e-10 rounds
+ * to 1e-10).  The records of the original text are then written with those scores (recalibrate_genotype: PL / GQ / GT
+ * from the W phreds) and BGZF-compressed; the outputs are those of ugvc_filter_bgzf_edits (edits->with_model must be 1).
+ * out_split[0..6] = out[0..6] of ugvc_ma_build; out_split[7] = 0, or with UGVC_E_DATA where the reference raises:
+ * 1 = the split build (a group, see ugvc_ma_data_error, or a contig without multi-allelic sites (out_split[0] = 0) or
+ * without deletion clusters (out_split[1] = 0)), 2 = the merge (a 2-class model).  UGVC_E_DATA with out_split[7] = 0
+ * is a data error of K1 (ugvc_last_data_error).  UGVC_E_FALLBACK (nothing written) where ugvc_filter_bgzf_edits falls
+ * back, and for a contig beyond the path's limits: text of 4 GiB or more, or larger than the reserved lanes of ctx /
+ * index_ctx.  Needs ugvc_enable_phreds(ctx, 2) before ugvc_reserve, and ctx, index_ctx and ma on one device. */
+int ugvc_filter_bgzf_split(ugvc_ctx* ctx, ugvc_ctx* index_ctx, ugvc_ma* ma, int lane, const uint8_t* bgzf, size_t n_bytes,
+                           uint32_t skip_head, uint64_t take_bytes, const uint8_t* ref_seq, size_t ref_len, double threshold, int flags,
+                           ugvc_file_edits* edits, uint8_t* out_bgzf, size_t out_capacity, size_t* out_bytes, uint32_t* out_block_csize,
+                           size_t block_capacity, size_t* out_n_blocks, ugvc_recinfo* out_recinfo, int64_t* out_line_start,
+                           uint8_t* out_low_score, size_t capacity_records, int64_t* out_n_records, int64_t out_split[8]);
+/* Stage times of the last ugvc_filter_bgzf_split call on `lane`, ms between CUDA events on its stream: H2D + inflate,
+ * index K1, split build, scored K1..K3, merge + score, record writer, deflate + pack, D2H.  The split build and the
+ * merge wait on the stream for their counts, so their stages include that host round trip. */
+int ugvc_filter_bgzf_split_stage_ms(ugvc_ctx* ctx, int lane, float out_ms[8]);
+/* Test hook: the score kernel of ugvc_filter_bgzf_split (ma_score) on n caller rows of `width` (>= 2) likelihoods:
+ * out_phreds[n][width], out_qual[n], out_low[n]. */
+int ugvc_test_ma_score(ugvc_ctx* ctx, const double* lik, int64_t n, int width, double threshold, double* out_phreds,
+                       double* out_qual, uint8_t* out_low);
 
 /* ---- test hook ------------------------------------------------------------ */
 /* K1's numeric-literal parser (csrc/numparse.h) compiled for the host: parses one token of

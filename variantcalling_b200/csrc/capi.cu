@@ -13,6 +13,7 @@
 #include "deflate.cuh"
 #ifndef UGVC_HOST_EMU
 #include "fileio.cuh"
+#include "multiallelic.cuh"
 #endif
 
 #define UGVC_VERSION 100
@@ -66,6 +67,8 @@ struct Lane {
         std::vector<uint32_t> h_bsize;
         cudaEvent_t ev[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
         float ms[5] = {0, 0, 0, 0, 0};
+        cudaEvent_t ev_split[9] = {};  // ugvc_filter_bgzf_split: created at its first call on the lane
+        float ms_split[8] = {0, 0, 0, 0, 0, 0, 0, 0};
     } fb;
 };
 
@@ -186,6 +189,8 @@ static void free_lane(Lane& l) {
     cudaFree(l.fb.d_bl_meta);
     if (l.fb.h_total) cudaFreeHost(l.fb.h_total);
     for (auto& e : l.fb.ev)
+        if (e) cudaEventDestroy(e);
+    for (auto& e : l.fb.ev_split)
         if (e) cudaEventDestroy(e);
     if (l.h_inf_err) cudaFreeHost(l.h_inf_err);
     if (l.h_n) cudaFreeHost(l.h_n);
@@ -1342,6 +1347,15 @@ extern "C" int64_t ugvc_test_write_records(ugvc_ctx* ctx, const uint8_t*, size_t
                                        int64_t*) {
     return fail(ctx, UGVC_E_STATE, "the device-side record writer is not part of the host emulation");
 }
+extern "C" int ugvc_filter_bgzf_split(ugvc_ctx* ctx, ugvc_ctx*, ugvc_ma*, int, const uint8_t*, size_t, uint32_t, uint64_t,
+                                      const uint8_t*, size_t, double, int, ugvc_file_edits*, uint8_t*, size_t, size_t*, uint32_t*,
+                                      size_t, size_t*, ugvc_recinfo*, int64_t*, uint8_t*, size_t, int64_t*, int64_t*) {
+    return fail(ctx, UGVC_E_FALLBACK, "the device split path is not part of the host emulation");
+}
+extern "C" int ugvc_filter_bgzf_split_stage_ms(ugvc_ctx*, int, float*) { return UGVC_E_FALLBACK; }
+extern "C" int ugvc_test_ma_score(ugvc_ctx* ctx, const double*, int64_t, int, double, double*, double*, uint8_t*) {
+    return fail(ctx, UGVC_E_STATE, "ma_score is not part of the host emulation");
+}
 extern "C" int ugvc_filter_bgzf_stage_ms(ugvc_ctx*, int, float*) { return UGVC_E_STATE; }
 extern "C" int ugvc_filter_bgzf_first_records(ugvc_ctx*, int, const uint64_t*, int, int64_t*) { return UGVC_E_STATE; }
 extern "C" int ugvc_test_device_deflate(ugvc_ctx* ctx, const uint8_t*, size_t, int, uint8_t*, size_t, uint32_t*, size_t, size_t*,
@@ -1621,6 +1635,189 @@ extern "C" int ugvc_filter_bgzf(ugvc_ctx* ctx, int lane, const uint8_t* bgzf, si
     return ugvc_filter_bgzf_edits(ctx, lane, bgzf, n_bytes, skip_head, take_bytes, threshold, flags, &e, out_bgzf, out_capacity,
                                   out_bytes, out_block_csize, block_capacity, out_n_blocks, out_recinfo, out_line_start,
                                   out_low_score, capacity_records, out_n_records);
+}
+
+// --treat_multiallelics on the file path: one whole contig a call, every stage on `lane`'s stream and device pointers.
+extern "C" int ugvc_filter_bgzf_split(ugvc_ctx* ctx, ugvc_ctx* index_ctx, ugvc_ma* ma, int lane, const uint8_t* bgzf, size_t n_bytes,
+                                      uint32_t skip_head, uint64_t take_bytes, const uint8_t* ref_seq, size_t ref_len, double threshold,
+                                      int flags, ugvc_file_edits* edits, uint8_t* out_bgzf, size_t out_capacity, size_t* out_bytes,
+                                      uint32_t* out_block_csize, size_t block_capacity, size_t* out_n_blocks, ugvc_recinfo* out_recinfo,
+                                      int64_t* out_line_start, uint8_t* out_low_score, size_t capacity_records, int64_t* out_n_records,
+                                      int64_t out_split[8]) {
+    if (!ctx) return UGVC_E_ARG;
+    if (!edits || !index_ctx || !ma || !out_split) return fail(ctx, UGVC_E_ARG, "filter_bgzf_split: NULL argument");
+    const ugvc_file_edits& e = *edits;
+    edits->n_blacklisted = 0;
+    memset(out_split, 0, 8 * sizeof(int64_t));
+    if (!ctx->has_plan || ctx->lanes.empty() || !index_ctx->has_plan || index_ctx->lanes.empty())
+        return fail(ctx, UGVC_E_STATE, "filter_bgzf_split: load the plans and reserve both contexts first");
+    if (ctx->plan.h.model_kind == MODEL_NONE || index_ctx->plan.h.model_kind != MODEL_NONE)
+        return fail(ctx, UGVC_E_STATE, "filter_bgzf_split: ctx needs a plan with a model, index_ctx the model-less plan");
+    if (ctx->want_phreds != 2) return fail(ctx, UGVC_E_STATE, "filter_bgzf_split: needs ugvc_enable_phreds(ctx, 2) before ugvc_reserve");
+    if (!e.with_model) return fail(ctx, UGVC_E_ARG, "filter_bgzf_split: the split branch scores with a model (with_model = 1)");
+    if (index_ctx->device != ctx->device || ma_device_of(ma) != ctx->device)
+        return fail(ctx, UGVC_E_ARG, "filter_bgzf_split: ctx, index_ctx and the split handle must share a device");
+    if (lane < 0 || lane >= (int)ctx->lanes.size() || lane >= (int)index_ctx->lanes.size())
+        return fail(ctx, UGVC_E_ARG, "filter_bgzf_split: lane out of range");
+    if (!bgzf || !n_bytes || !out_bgzf || !out_bytes || !out_n_records || (ref_len && !ref_seq))
+        return fail(ctx, UGVC_E_ARG, "filter_bgzf_split: NULL argument");
+    CU(cudaSetDevice(ctx->device));
+    Lane& l = ctx->lanes[lane];
+    Lane& il = index_ctx->lanes[lane];
+    if (l.submitted || il.submitted) return fail(ctx, UGVC_E_STATE, "filter_bgzf_split: lane already has a batch in flight");
+    int rc = file_bufs(ctx, l);
+    if (rc) return rc;
+    Lane::FileBufs& f = l.fb;
+    if (!f.ev_split[0])
+        for (auto& ev : f.ev_split) CU(cudaEventCreate(&ev));
+    cudaStream_t st = l.stream;
+    (void)cudaGetLastError();
+    FioEdits ed{};
+    ed.with_model = 1;
+    ed.flags = flags;
+    ed.bl_mask = f.d_bl_mask;
+    ed.n_blacklisted = f.d_n_bl;
+    ed.out_end = e.out_end ? f.d_end : nullptr;
+    rc = upload_blacklists(ctx, f, e, ed, st);
+    if (rc) return rc;
+    CU(cudaEventRecord(f.ev_split[0], st));
+    // ---- compressed blocks -> text on the device, the contig's first byte 16-byte aligned
+    const size_t shift = (16 - (skip_head & 15u)) & 15u;
+    size_t total = 0;
+    rc = stage_bgzf(ctx, l, bgzf, n_bytes, inflate_decoder(), &total, shift);
+    if (rc) return rc;
+    if (skip_head > total) return fail(ctx, UGVC_E_ARG, "filter_bgzf_split: skip_head beyond the inflated blocks");
+    const size_t n_text = take_bytes ? (size_t)take_bytes : total - skip_head;
+    if (skip_head + n_text > total) return fail(ctx, UGVC_E_ARG, "filter_bgzf_split: the range is longer than the inflated blocks");
+    if (n_text >= (1ull << 32) - 64u || n_text > index_ctx->cap_bytes)
+        return fail(ctx, UGVC_E_FALLBACK, "filter_bgzf_split: the contig is beyond the device split's limits");
+    const uint8_t* d_text = l.d_text + shift + skip_head;
+    CU(cudaEventRecord(f.ev_split[1], st));
+    // ---- index pass: K1 of the model-less plan into the index context's lane (the scored pass leaves them alone)
+    rc = enqueue_kernels(index_ctx, il, d_text, n_text, threshold, il.b.low_score, il.b.probs, il.b.qual, il.b.recinfo, il.b.line_start,
+                         il.b.cap_records, il.b.n_records, st);
+    if (rc) return fail(ctx, rc, index_ctx->err);
+    CU(cudaMemcpyAsync(il.h_n, il.b.n_records, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(il.h_err, il.d_err, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+    CU(cudaEventRecord(f.ev_split[2], st));
+    CU(cudaStreamSynchronize(st));
+    if (l.h_inf_err && *l.h_inf_err) {
+        const int code = *l.h_inf_err;
+        *l.h_inf_err = 0;
+        return fail(ctx, UGVC_E_IO, inf_err_message(code));
+    }
+    rc = decode_error(index_ctx, *il.h_err);
+    if (rc) return fail(ctx, rc, index_ctx->err);
+    const int64_t n = *il.h_n;
+    il.last_n = n;
+    *out_n_records = n;
+    if ((size_t)n > capacity_records) return fail(ctx, UGVC_E_ARG, "filter_bgzf_split: output capacity smaller than the record count");
+    if ((size_t)n > l.b.cap_records) return fail(ctx, UGVC_E_FALLBACK, "filter_bgzf_split: more records than the reserved lane holds");
+    // ---- split build (UGVC_E_DATA: the reference raises on this contig; out_split[7] = 1)
+    rc = ma_build_on(ma, d_text, n_text, il.b.line_start, il.b.recinfo, n, ref_seq, ref_len, st, out_split);
+    if (rc == UGVC_OK && (out_split[0] == 0 || out_split[1] == 0)) {
+        rc = UGVC_E_DATA;  // no multi-allelic site / no deletion cluster on the contig: the reference raises before scoring
+        ctx->err = "the reference raises on this contig (no multi-allelic site or no deletion cluster)";
+    } else if (rc) {
+        ctx->err = ugvc_ma_last_error(ma);
+    }
+    if (rc == UGVC_E_DATA) out_split[7] = 1;
+    if (rc) return rc;
+    CU(cudaEventRecord(f.ev_split[3], st));
+    // ---- scored pass: K1..K3 on the kept lines and split rows, fp64 likelihoods into the lane's phred buffer
+    const int64_t n_scored = out_split[2] + out_split[3];
+    const size_t scored_bytes = (size_t)(out_split[4] + out_split[5]);
+    if (scored_bytes > ctx->cap_bytes || (size_t)n_scored > l.b.cap_records)
+        return fail(ctx, UGVC_E_FALLBACK, "filter_bgzf_split: the scored text is larger than the reserved lane");
+    uint8_t* d_scored = ma_scored_text(ma);
+    CU(cudaMemsetAsync(d_scored + scored_bytes, '\n', TEXT_SLACK, st));
+    rc = enqueue_kernels(ctx, l, d_scored, scored_bytes, threshold, l.b.low_score, l.b.probs, l.b.qual, l.b.recinfo, l.b.line_start,
+                         l.b.cap_records, l.b.n_records, st);
+    if (rc) return rc;
+    CU(cudaMemcpyAsync(l.h_n, l.b.n_records, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(l.h_err, l.d_err, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+    CU(cudaEventRecord(f.ev_split[4], st));
+    // ---- merge (synchronises the stream), then the score math over the N x W matrix; the phreds overwrite it in place
+    const int K = ctx->plan.h.n_classes;
+    const int W = (int)(out_split[6] > K ? out_split[6] : K);
+    double* d_mat = nullptr;
+    const int rc_merge = ma_merge_on(ma, l.b.phreds, n_scored, K, W, st, &d_mat);
+    CU(cudaStreamSynchronize(st));  // (already done unless the merge refused its arguments)
+    rc = decode_error(ctx, *l.h_err);  // a data error of the scored pass comes first, as on the host path
+    if (rc) return rc;
+    if (*l.h_n != n_scored) return fail(ctx, UGVC_E_STATE, "filter_bgzf_split: the scored pass read an unexpected number of rows");
+    if (rc_merge == UGVC_E_DATA) out_split[7] = 2;
+    if (rc_merge) return fail(ctx, rc_merge, ugvc_ma_last_error(ma));
+    ma_launch_score(d_mat, n, W, threshold, e.recalibrate_genotype ? d_mat : nullptr, l.b.qual, l.b.low_score, ctx->sm_count, st);
+    CU(cudaGetLastError());
+    CU(cudaEventRecord(f.ev_split[5], st));
+    // ---- record writer over the original text and the index pass's records
+    ed.phreds = e.recalibrate_genotype ? d_mat : nullptr;
+    ed.n_classes = W;
+    size_t out_text = 0;
+    rc = write_records(ctx, f, d_text, il.b.line_start, il.b.recinfo, l.b.low_score, l.b.qual, n, ed, st, &out_text);
+    if (rc) return rc;
+    CU(cudaEventRecord(f.ev_split[6], st));
+    // ---- deflate, pack
+    const int n_blocks = (int)((out_text + DEF_CHUNK - 1) / DEF_CHUNK);
+    if ((size_t)n_blocks > f.cap_blocks || (out_block_csize && (size_t)n_blocks > block_capacity))
+        return fail(ctx, UGVC_E_ARG, "filter_bgzf_split: more output blocks than room for them");
+    rc = encode_blocks(ctx, f, out_text, n_blocks, deflate_encoder(), st);
+    if (rc) return rc;
+    f.h_bsize.resize((size_t)n_blocks + 1);
+    if (n_blocks) CU(cudaMemcpyAsync(f.h_bsize.data(), f.d_bsize, (size_t)n_blocks * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+    CU(cudaEventRecord(f.ev_split[7], st));
+    CU(cudaStreamSynchronize(st));
+    if (*f.h_fallback) return UGVC_E_FALLBACK;
+    size_t packed = 0;
+    for (int b = 0; b < n_blocks; ++b) packed += f.h_bsize[b];
+    if (packed > out_capacity) return fail(ctx, UGVC_E_FALLBACK, "filter_bgzf_split: out_capacity smaller than the compressed output");
+    ctx->launches += 7;
+    // ---- results to the host
+    if (packed) CU(cudaMemcpyAsync(out_bgzf, f.d_packed, packed, cudaMemcpyDeviceToHost, st));
+    if (out_block_csize && n_blocks) memcpy(out_block_csize, f.h_bsize.data(), (size_t)n_blocks * sizeof(uint32_t));
+    if (out_recinfo && n) CU(cudaMemcpyAsync(out_recinfo, il.b.recinfo, (size_t)n * sizeof(ugvc_recinfo), cudaMemcpyDeviceToHost, st));
+    if (out_line_start) CU(cudaMemcpyAsync(out_line_start, f.d_out_ls, (size_t)(n + 1) * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    if (out_low_score && n) CU(cudaMemcpyAsync(out_low_score, l.b.low_score, (size_t)n, cudaMemcpyDeviceToHost, st));
+    if (e.out_end && n) CU(cudaMemcpyAsync(e.out_end, f.d_end, (size_t)n * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    CU(cudaEventRecord(f.ev_split[8], st));
+    CU(cudaStreamSynchronize(st));
+    *out_bytes = packed;
+    edits->n_blacklisted = (int64_t)*f.h_n_bl;
+    if (out_n_blocks) *out_n_blocks = (size_t)n_blocks;
+    for (int k = 0; k < 8; ++k) cudaEventElapsedTime(&f.ms_split[k], f.ev_split[k], f.ev_split[k + 1]);
+    return UGVC_OK;
+}
+
+extern "C" int ugvc_filter_bgzf_split_stage_ms(ugvc_ctx* ctx, int lane, float out_ms[8]) {
+    if (!ctx || !out_ms || lane < 0 || lane >= (int)ctx->lanes.size()) return UGVC_E_ARG;
+    for (int k = 0; k < 8; ++k) out_ms[k] = ctx->lanes[lane].fb.ms_split[k];
+    return UGVC_OK;
+}
+
+extern "C" int ugvc_test_ma_score(ugvc_ctx* ctx, const double* lik, int64_t n, int width, double threshold, double* out_phreds,
+                                  double* out_qual, uint8_t* out_low) {
+    // test hook: ma_score (csrc/multiallelic.cu) on the caller's rows of `width` likelihoods
+    if (!ctx || n < 0 || width < 2 || (n && (!lik || !out_phreds || !out_qual || !out_low))) return UGVC_E_ARG;
+    if (n == 0) return UGVC_OK;
+    CU(cudaSetDevice(ctx->device));
+    struct DevFree {
+        void* p = nullptr;
+        ~DevFree() { cudaFree(p); }
+    } d_lik, d_ph, d_q, d_low;
+    const size_t cells = (size_t)n * width;
+    CU(cudaMalloc(&d_lik.p, cells * sizeof(double)));
+    CU(cudaMalloc(&d_ph.p, cells * sizeof(double)));
+    CU(cudaMalloc(&d_q.p, (size_t)n * sizeof(double)));
+    CU(cudaMalloc(&d_low.p, (size_t)n));
+    CU(cudaMemcpy(d_lik.p, lik, cells * sizeof(double), cudaMemcpyHostToDevice));
+    ma_launch_score(static_cast<const double*>(d_lik.p), n, width, threshold, static_cast<double*>(d_ph.p), static_cast<double*>(d_q.p),
+                    static_cast<uint8_t*>(d_low.p), ctx->sm_count, nullptr);
+    CU(cudaGetLastError());
+    CU(cudaMemcpy(out_phreds, d_ph.p, cells * sizeof(double), cudaMemcpyDeviceToHost));
+    CU(cudaMemcpy(out_qual, d_q.p, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost));
+    CU(cudaMemcpy(out_low, d_low.p, (size_t)n, cudaMemcpyDeviceToHost));
+    return UGVC_OK;
 }
 
 extern "C" int64_t ugvc_test_write_records(ugvc_ctx* ctx, const uint8_t* text, size_t n_bytes, const int64_t* line_start,

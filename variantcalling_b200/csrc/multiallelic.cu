@@ -19,6 +19,8 @@
 //                     the two haplotypes in the +-20 bp reference window, VARIANT_TYPE / QUAL / GQ / QD recomputed
 //   ma_copy_kept      the untouched lines, compacted in input order in front of the rows
 //   ma_merge          one thread per record: likelihoods of the scored pass -> N x W matrix in input record order
+//   ma_score          one thread per record: phreds / qual / LOW_SCORE of the merged matrix (the device file path,
+//                     ugvc_filter_bgzf_split; the host path does this step in NumPy)
 //
 // The rows are TEXT on purpose: the scored pass then runs the ordinary K1..K3 kernels on them, so the split rows
 // get the features any record gets.  Every kernel is a grid-stride loop (shared memory only stages copies), so the host
@@ -33,6 +35,7 @@
 #include <string>
 
 #include "../../include/ugvc_b200.h"
+#include "multiallelic.cuh"
 
 #define MA_MAX_ALLELES 32
 #define MA_CHUNK 256
@@ -1436,6 +1439,35 @@ __global__ void ma_merge(int64_t n, const int64_t* __restrict__ rec_row, const M
         o[ma_pl_idx(i2, i2)] = __dmul_rn(s0[2], s1[2]);
     }
 }
+// -10 log10(lik + 1e-10).  The sum is the double nearest 1e-10 for lik = 0 (the literal 0.0 ma_merge writes, the 0 / 1
+// probabilities of a random forest) and anything below 1e-26: its log10 lies 2^-56 from -10, which NumPy rounds to -10
+// and so prints PL 100, while a log10 one ulp short of -10 would print 99.  That case is exact; any other value is CUDA's
+// log10, within an ulp of NumPy's (DESIGN.md section 4).
+__device__ __forceinline__ double ma_phred(double lik) {
+    const double x = __dadd_rn(lik, 1e-10);
+    return x == 1e-10 ? 100.0 : __dmul_rn(-10.0, log10(x));
+}
+// multiallelics.score_math (filter_variants_pipeline.py:174-180,192) over the merged N x W matrix, one thread per record:
+// phreds of all W columns (the zero padding included, as NumPy's min over ph[1:] sees it), qual = max(30 + ph0 -
+// min(ph[1:]), 0) summed in K3's order, low = qual <= threshold.  phreds may alias lik (a thread rewrites its own row).
+__global__ void ma_score(const double* lik, int64_t n, int W, double threshold, double* phreds, double* __restrict__ qual,
+                         uint8_t* __restrict__ low) {
+    for (int64_t i = MA_TID; i < n; i += MA_NTHREADS) {
+        const double* r = lik + i * W;
+        double* o = phreds ? phreds + i * W : nullptr;
+        double ph0 = 0.0, mn = 0.0;
+        for (int k = 0; k < W; ++k) {
+            const double p = ma_phred(r[k]);
+            if (o) o[k] = p;
+            if (k == 0) ph0 = p;
+            else if (k == 1 || p < mn) mn = p;
+        }
+        double q = __dadd_rn(__dadd_rn(30.0, ph0), -mn);
+        q = q < 0.0 ? 0.0 : q;
+        qual[i] = q;
+        low[i] = q <= threshold ? 1 : 0;
+    }
+}
 
 // ---------------------------------------------------------------------------------------------------
 // C ABI (include/ugvc_b200.h)
@@ -1545,25 +1577,10 @@ extern "C" int ugvc_ma_set_rules(ugvc_ma* h, const void* blob, size_t n_bytes) {
     return UGVC_OK;
 }
 
-// One contig: text + the index pass's line starts / recinfo + the contig's reference sequence -> groups, split rows,
-// the text of the scored pass.  out[0..7] = {n_singles, n_cluster_records, n_kept_records, n_rows, kept_bytes,
-// rows_bytes, width of the widest two-row group's genotype vector, 0}.  UGVC_E_DATA: a group the reference raises
-// on (ugvc_ma_data_error tells which and why).
-extern "C" int ugvc_ma_build(ugvc_ma* h, const uint8_t* text, size_t n_bytes, const int64_t* line_start, const ugvc_recinfo* recinfo,
-                             int64_t n_records, const uint8_t* ref_seq, size_t ref_len, int64_t out[8]) {
-    if (!h || !out || (n_bytes && !text) || !line_start || (n_records && !recinfo) || (ref_len && !ref_seq) || n_records < 0)
-        return ma_fail(h, UGVC_E_ARG, "ma_build: bad arguments");
-    if (!h->has_rules) return ma_fail(h, UGVC_E_STATE, "ma_build: set the rules first");
-    if (n_bytes >= (1ull << 32) - 64u) return ma_fail(h, UGVC_E_ARG, "ma_build: a contig's text must stay below 4 GiB");
-    MA_CU(cudaSetDevice(h->device));
-    const int64_t n = n_records, n_chunks = (n + MA_CHUNK - 1) / MA_CHUNK;
-    cudaStream_t st = h->stream;
-    h->n = n;
-    h->last_err = ~0ull;
-    memset(out, 0, 8 * sizeof(int64_t));
+// the per-record scratch of a contig of n records and its reference sequence, grown on demand
+static int ma_reserve(ugvc_ma* h, int64_t n, size_t ref_len) {
     {
         size_t c;
-        c = h->cap_bytes; MA_CU(ma_grow(&h->d_text, &c, n_bytes + 64, n_bytes / 8)); h->cap_bytes = c;
         c = h->cap_ref; MA_CU(ma_grow(&h->d_ref, &c, ref_len + 64, 0)); h->cap_ref = c;
         if ((size_t)n + 1 > h->cap_records) {
             const size_t cap = (size_t)n + 1 + (size_t)n / 8;
@@ -1586,10 +1603,25 @@ extern "C" int ugvc_ma_build(ugvc_ma* h, const uint8_t* text, size_t n_bytes, co
             h->cap_records = cap;
         }
     }
+    return UGVC_OK;
+}
+
+int ma_build_on(ugvc_ma* h, const uint8_t* d_text, size_t n_bytes, const int64_t* d_line_start, const ugvc_recinfo* d_recinfo,
+                int64_t n_records, const uint8_t* ref_seq, size_t ref_len, cudaStream_t st, int64_t out[8]) {
+    if (!h || !out || (n_bytes && !d_text) || !d_line_start || (n_records && !d_recinfo) || (ref_len && !ref_seq) || n_records < 0)
+        return ma_fail(h, UGVC_E_ARG, "ma_build: bad arguments");
+    if (!h->has_rules) return ma_fail(h, UGVC_E_STATE, "ma_build: set the rules first");
+    if (n_bytes >= (1ull << 32) - 64u) return ma_fail(h, UGVC_E_ARG, "ma_build: a contig's text must stay below 4 GiB");
+    MA_CU(cudaSetDevice(h->device));
+    const int64_t n = n_records, n_chunks = (n + MA_CHUNK - 1) / MA_CHUNK;
+    h->n = n;
+    h->n_groups = h->n_singles = h->n_kept = h->n_rows = h->kept_bytes = h->rows_bytes = 0;
+    h->width_groups = 0;
+    h->last_err = ~0ull;
+    memset(out, 0, 8 * sizeof(int64_t));
+    int rc = ma_reserve(h, n, ref_len);
+    if (rc) return rc;
     if (n == 0) return UGVC_OK;
-    MA_CU(cudaMemcpyAsync(h->d_text, text, n_bytes, cudaMemcpyHostToDevice, st));
-    MA_CU(cudaMemcpyAsync(h->d_line_start, line_start, ((size_t)n + 1) * sizeof(int64_t), cudaMemcpyHostToDevice, st));
-    MA_CU(cudaMemcpyAsync(h->d_recinfo, recinfo, (size_t)n * sizeof(ugvc_recinfo), cudaMemcpyHostToDevice, st));
     if (ref_len) MA_CU(cudaMemcpyAsync(h->d_ref, ref_seq, ref_len, cudaMemcpyHostToDevice, st));
     MA_CU(cudaMemsetAsync(h->d_head_mark, 0, (size_t)n, st));
     int64_t init[16];
@@ -1604,15 +1636,15 @@ extern "C" int ugvc_ma_build(ugvc_ma* h, const uint8_t* text, size_t n_bytes, co
     const int tpb = 256;
     const int grid_rec = (int)((n + tpb - 1) / tpb < (int64_t)h->sm_count * 8 ? (n + tpb - 1) / tpb : (int64_t)h->sm_count * 8);
     const int grid_chunk = (int)((n_chunks + 63) / 64 < (int64_t)h->sm_count * 8 ? (n_chunks + 63) / 64 : (int64_t)h->sm_count * 8);
-    MA_LAUNCH(ma_scan_alleles, grid_rec, tpb, st, h->d_text, h->d_line_start, h->d_recinfo, n, h->d_key, h->d_flags, d_first);
+    MA_LAUNCH(ma_scan_alleles, grid_rec, tpb, st, d_text, d_line_start, d_recinfo, n, h->d_key, h->d_flags, d_first);
     MA_LAUNCH(ma_reach_agg, grid_chunk, 64, st, h->d_key, n, d_first, h->d_agg);
     MA_LAUNCH(ma_spine_max, 1, 1, st, h->d_agg, n_chunks);
     int64_t* d_head_agg = h->d_agg4;  // (free until ma_groups_agg)
-    MA_LAUNCH(ma_reach_apply, grid_chunk, 64, st, h->d_key, h->d_recinfo, n, d_first, h->d_agg, h->d_flags, d_head_agg);
+    MA_LAUNCH(ma_reach_apply, grid_chunk, 64, st, h->d_key, d_recinfo, n, d_first, h->d_agg, h->d_flags, d_head_agg);
     MA_LAUNCH(ma_spine_max, 1, 1, st, d_head_agg, n_chunks);
     MA_LAUNCH(ma_owner_apply, grid_chunk, 64, st, n, d_first, d_head_agg, h->d_flags, h->d_owner, h->d_scalars + 6);
     MA_LAUNCH(ma_mark_heads, grid_rec, tpb, st, n, h->d_owner, h->d_head_mark);
-    MA_LAUNCH(ma_groups_agg, grid_chunk, 64, st, n, h->d_line_start, h->d_owner, h->d_head_mark, h->d_scalars + 6, h->d_flags, h->d_agg4);
+    MA_LAUNCH(ma_groups_agg, grid_chunk, 64, st, n, d_line_start, h->d_owner, h->d_head_mark, h->d_scalars + 6, h->d_flags, h->d_agg4);
     MA_LAUNCH(ma_spine_sum4, 1, 1, st, h->d_agg4, n_chunks, h->d_scalars);
     h->launches += 9;
     int64_t totals[16];
@@ -1628,7 +1660,7 @@ extern "C" int ugvc_ma_build(ugvc_ma* h, const uint8_t* text, size_t n_bytes, co
         MA_CU(ma_grow(&h->d_groups, &c, (size_t)h->n_groups + 1, (size_t)h->n_groups / 4));
         h->cap_groups = c;
     }
-    MA_LAUNCH(ma_groups_apply, grid_chunk, 64, st, n, h->d_line_start, h->d_owner, h->d_flags, h->d_recinfo, h->d_agg4, h->d_scalars,
+    MA_LAUNCH(ma_groups_apply, grid_chunk, 64, st, n, d_line_start, h->d_owner, h->d_flags, d_recinfo, h->d_agg4, h->d_scalars,
               h->d_groups, h->d_kept_off, h->d_rec_row);
     // a warp per group
     const int64_t grp_ctas = (h->n_groups + MA_ROW_WARPS - 1) / MA_ROW_WARPS;
@@ -1637,7 +1669,7 @@ extern "C" int ugvc_ma_build(ugvc_ma* h, const uint8_t* text, size_t n_bytes, co
     const int64_t grp_chunks = (h->n_groups + MA_CHUNK - 1) / MA_CHUNK;
     const int grid_gchunk = (int)((grp_chunks + 63) / 64 > 0 ? (grp_chunks + 63) / 64 : 1);
     if (h->n_groups) {
-        MA_LAUNCH(ma_plan_rows, grid_grp, row_tpb, st, h->d_text, h->d_line_start, h->rules, h->d_ref, (int64_t)ref_len, h->d_groups, h->n_groups,
+        MA_LAUNCH(ma_plan_rows, grid_grp, row_tpb, st, d_text, d_line_start, h->rules, h->d_ref, (int64_t)ref_len, h->d_groups, h->n_groups,
                   d_err, d_width);
         MA_LAUNCH(ma_rowoff_agg, grid_gchunk, 64, st, h->d_groups, h->n_groups, h->d_agg4);
         h->launches += 2;
@@ -1668,9 +1700,9 @@ extern "C" int ugvc_ma_build(ugvc_ma* h, const uint8_t* text, size_t n_bytes, co
         h->cap_out = c;
     }
     const int grid_copy = (int)(n_chunks < (int64_t)h->sm_count * 16 ? n_chunks : (int64_t)h->sm_count * 16);  // a CTA per chunk of records
-    MA_LAUNCH(ma_copy_kept, grid_copy, 128, st, h->d_text, h->d_line_start, h->d_kept_off, n, h->d_out);
+    MA_LAUNCH(ma_copy_kept, grid_copy, 128, st, d_text, d_line_start, h->d_kept_off, n, h->d_out);
     if (h->n_groups) {
-        MA_LAUNCH(ma_write_rows, grid_grp, row_tpb, st, h->d_text, h->d_line_start, h->rules, h->d_ref, (int64_t)ref_len, h->d_groups, h->n_groups,
+        MA_LAUNCH(ma_write_rows, grid_grp, row_tpb, st, d_text, d_line_start, h->rules, h->d_ref, (int64_t)ref_len, h->d_groups, h->n_groups,
                   h->d_out + h->kept_bytes);
         h->launches += 1;
     }
@@ -1679,6 +1711,34 @@ extern "C" int ugvc_ma_build(ugvc_ma* h, const uint8_t* text, size_t n_bytes, co
     MA_CU(cudaGetLastError());
     if (h->last_err != ~0ull) return ma_fail(h, UGVC_E_DATA, "a record the reference raises on (ugvc_ma_data_error)");
     return UGVC_OK;
+}
+uint8_t* ma_scored_text(ugvc_ma* h) { return h->d_out; }
+int ma_device_of(const ugvc_ma* h) { return h->device; }
+
+// One contig: text + the index pass's line starts / recinfo + the contig's reference sequence -> groups, split rows,
+// the text of the scored pass.  out[0..7] = {n_singles, n_cluster_records, n_kept_records, n_rows, kept_bytes,
+// rows_bytes, width of the widest two-row group's genotype vector, 0}.  UGVC_E_DATA: a group the reference raises
+// on (ugvc_ma_data_error tells which and why).  The host inputs are copied to the handle's buffers, then ma_build_on.
+extern "C" int ugvc_ma_build(ugvc_ma* h, const uint8_t* text, size_t n_bytes, const int64_t* line_start, const ugvc_recinfo* recinfo,
+                             int64_t n_records, const uint8_t* ref_seq, size_t ref_len, int64_t out[8]) {
+    if (!h || !out || (n_bytes && !text) || !line_start || (n_records && !recinfo) || (ref_len && !ref_seq) || n_records < 0)
+        return ma_fail(h, UGVC_E_ARG, "ma_build: bad arguments");
+    if (n_bytes >= (1ull << 32) - 64u) return ma_fail(h, UGVC_E_ARG, "ma_build: a contig's text must stay below 4 GiB");
+    MA_CU(cudaSetDevice(h->device));
+    cudaStream_t st = h->stream;
+    {
+        size_t c = h->cap_bytes;
+        MA_CU(ma_grow(&h->d_text, &c, n_bytes + 64, n_bytes / 8));
+        h->cap_bytes = c;
+    }
+    int rc = ma_reserve(h, n_records, ref_len);
+    if (rc) return rc;
+    if (n_records) {
+        MA_CU(cudaMemcpyAsync(h->d_text, text, n_bytes, cudaMemcpyHostToDevice, st));
+        MA_CU(cudaMemcpyAsync(h->d_line_start, line_start, ((size_t)n_records + 1) * sizeof(int64_t), cudaMemcpyHostToDevice, st));
+        MA_CU(cudaMemcpyAsync(h->d_recinfo, recinfo, (size_t)n_records * sizeof(ugvc_recinfo), cudaMemcpyHostToDevice, st));
+    }
+    return ma_build_on(h, h->d_text, n_bytes, h->d_line_start, h->d_recinfo, n_records, ref_seq, ref_len, st, out);
 }
 // detail of the last UGVC_E_DATA: group index (singles first, then cluster records), its record, the MA_E_* code
 extern "C" int ugvc_ma_data_error(const ugvc_ma* h, int64_t* group, int32_t* code) {
@@ -1717,28 +1777,24 @@ extern "C" int ugvc_ma_fetch(ugvc_ma* h, uint8_t* out_text, size_t capacity, int
     }
     return UGVC_OK;
 }
-// likelihoods of the scored pass (n_kept + n_rows rows of n_classes, row-major fp64) -> out[n_records][width],
-// width = max(n_classes, widest two-row group)
-extern "C" int ugvc_ma_merge(ugvc_ma* h, const double* lik, int64_t n_rows, int n_classes, double* out, int width) {
-    if (!h || !lik || !out || n_classes <= 0) return UGVC_E_ARG;
+int ma_merge_on(ugvc_ma* h, const double* d_lik, int64_t n_rows, int n_classes, int width, cudaStream_t st, double** d_mat) {
+    if (!h || !d_lik || !d_mat || n_classes <= 0) return ma_fail(h, UGVC_E_ARG, "ma_merge: bad arguments");
     if (n_rows != h->n_kept + h->n_rows) return ma_fail(h, UGVC_E_ARG, "ma_merge: the scored pass returned an unexpected number of rows");
     const int need = h->width_groups > n_classes ? h->width_groups : n_classes;
     if (width != need) return ma_fail(h, UGVC_E_ARG, "ma_merge: width must be max(n_classes, widest group)");
     MA_CU(cudaSetDevice(h->device));
-    cudaStream_t st = h->stream;
-    size_t c;
-    c = h->cap_lik; MA_CU(ma_grow(&h->d_lik, &c, (size_t)n_rows * n_classes + 8, 0)); h->cap_lik = c;
-    c = h->cap_mat; MA_CU(ma_grow(&h->d_mat, &c, (size_t)h->n * width + 8, 0)); h->cap_mat = c;
-    MA_CU(cudaMemcpyAsync(h->d_lik, lik, (size_t)n_rows * n_classes * sizeof(double), cudaMemcpyHostToDevice, st));
+    size_t c = h->cap_mat;
+    MA_CU(ma_grow(&h->d_mat, &c, (size_t)h->n * width + 8, 0));
+    h->cap_mat = c;
+    *d_mat = h->d_mat;
     const int64_t minus1 = -1;
     MA_CU(cudaMemcpyAsync(h->d_scalars + 8, &minus1, sizeof(minus1), cudaMemcpyHostToDevice, st));
     const int tpb = 256;
     const int grid = (int)((h->n + tpb - 1) / tpb < (int64_t)h->sm_count * 8 ? (h->n + tpb - 1) / tpb : (int64_t)h->sm_count * 8);
     if (h->n) {
-        MA_LAUNCH(ma_merge, grid, tpb, st, h->n, h->d_rec_row, h->d_groups, h->n_kept, h->d_lik, n_classes, h->d_mat, width,
+        MA_LAUNCH(ma_merge, grid, tpb, st, h->n, h->d_rec_row, h->d_groups, h->n_kept, d_lik, n_classes, h->d_mat, width,
                   reinterpret_cast<unsigned long long*>(h->d_scalars + 8));
         h->launches += 1;
-        MA_CU(cudaMemcpyAsync(out, h->d_mat, (size_t)h->n * width * sizeof(double), cudaMemcpyDeviceToHost, st));
     }
     int64_t errw = -1;
     MA_CU(cudaMemcpyAsync(&errw, h->d_scalars + 8, sizeof(errw), cudaMemcpyDeviceToHost, st));
@@ -1747,4 +1803,28 @@ extern "C" int ugvc_ma_merge(ugvc_ma* h, const double* lik, int64_t n_rows, int 
     h->last_err = (unsigned long long)errw;
     if (h->last_err != ~0ull) return ma_fail(h, UGVC_E_DATA, "a 2-class model cannot be merged over a split record");
     return UGVC_OK;
+}
+// likelihoods of the scored pass (n_kept + n_rows rows of n_classes, row-major fp64) -> out[n_records][width],
+// width = max(n_classes, widest two-row group).  The host likelihoods are copied to the handle's buffer, then ma_merge_on.
+extern "C" int ugvc_ma_merge(ugvc_ma* h, const double* lik, int64_t n_rows, int n_classes, double* out, int width) {
+    if (!h || !lik || !out || n_classes <= 0 || n_rows < 0) return UGVC_E_ARG;
+    MA_CU(cudaSetDevice(h->device));
+    cudaStream_t st = h->stream;
+    size_t c = h->cap_lik;
+    MA_CU(ma_grow(&h->d_lik, &c, (size_t)n_rows * n_classes + 8, 0));
+    h->cap_lik = c;
+    MA_CU(cudaMemcpyAsync(h->d_lik, lik, (size_t)n_rows * n_classes * sizeof(double), cudaMemcpyHostToDevice, st));
+    double* d_mat = nullptr;
+    const int rc = ma_merge_on(h, h->d_lik, n_rows, n_classes, width, st, &d_mat);
+    if (rc) return rc;
+    if (h->n) MA_CU(cudaMemcpy(out, d_mat, (size_t)h->n * width * sizeof(double), cudaMemcpyDeviceToHost));
+    return UGVC_OK;
+}
+
+void ma_launch_score(const double* lik, int64_t n, int width, double threshold, double* phreds, double* qual, uint8_t* low,
+                     int sm_count, cudaStream_t st) {
+    if (n <= 0) return;
+    const int tpb = 256;
+    const int grid = (int)((n + tpb - 1) / tpb < (int64_t)sm_count * 8 ? (n + tpb - 1) / tpb : (int64_t)sm_count * 8);
+    MA_LAUNCH(ma_score, grid, tpb, st, lik, n, width, threshold, phreds, qual, low);
 }

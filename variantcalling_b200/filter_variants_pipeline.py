@@ -20,7 +20,8 @@ written directly (the reference shells out to ``bcftools index -t``, :231).
 the first sample (:203-215).  ``--treat_multiallelics`` (:145-166): per contig, an index pass
 (K0+K1) finds the multi-allelic records and deletion clusters, their biallelic split rows are
 written as VCF lines (``variantcalling_b200/multiallelics.py``) and scored by the same kernels with
-the untouched records; the fp64 likelihoods are merged per record on the host.
+the untouched records; the fp64 likelihoods are merged per record.  On the device file path all of
+that runs in one call per contig (``ugvc_filter_bgzf_split``); ``--host_io`` merges and scores on the host.
 """
 from __future__ import annotations
 
@@ -559,10 +560,11 @@ def run(argv: list[str]):  # noqa: C901, PLR0912, PLR0915
         # compressed bytes both ways: the contig's BGZF blocks go to the device as they are, come back filtered, edited
         # and compressed again (ugvc_filter_bgzf_edits: with or without a model, blacklists, --recalibrate_genotype; the
         # writer also reads INFO/END, where the index ends a record when the header declares the tag, as htslib does).
-        # --treat_multiallelics keeps the host readers / writers: its index pass, split build and scored pass over a
-        # whole contig are not chained on the device
+        # --treat_multiallelics takes one whole contig a call through ugvc_filter_bgzf_split (index pass, split build,
+        # scored pass, merge and score math chained on the device); UGVC_MA_HOST=1 keeps it on the host readers / writers
         out.index_info_end = "END" in header.info
-        device_io = bool(not split_sites and not args.host_io)
+        split_device = bool(split_sites and not args.host_io and os.environ.get("UGVC_MA_HOST", "0") in ("", "0"))
+        device_io = bool((not split_sites or split_device) and not args.host_io)
         file_flags = (lib.FILE_OVERWRITE_QUAL if args.overwrite_qual_tag else 0) | \
                      (lib.FILE_BLACKLIST_CG if args.blacklist_cg_insertions else 0)
 
@@ -581,7 +583,7 @@ def run(argv: list[str]):  # noqa: C901, PLR0912, PLR0915
 
         in_pool, out_pool = _PinnedPool(3), _PinnedPool(3)  # two device calls in flight + the reader / the writer
         split_plans = [None]  # --treat_multiallelics: the device split plan, carried from contig to contig
-        dev_ms = np.zeros(5)
+        dev_ms = np.zeros(8)  # stage ms of the device calls (5 stages of ugvc_filter_bgzf_edits, 8 of ugvc_filter_bgzf_split)
 
         def host_contig(contig: str, loaded):
             """One contig through the host readers / writers (text inflated on the host, records spliced on host threads)."""
@@ -604,7 +606,7 @@ def run(argv: list[str]):  # noqa: C901, PLR0912, PLR0915
                 need_idx = (text.size + 4096, n_contig + 128)
                 if need_idx[0] > idx_reserved[0] or need_idx[1] > idx_reserved[1]:
                     idx_reserved = (max(need_idx[0], idx_reserved[0]), max(need_idx[1], idx_reserved[1]))
-                    idx_ctx.reserve(idx_reserved[0], idx_reserved[1], 1)
+                    idx_ctx.reserve(idx_reserved[0], idx_reserved[1], n_lanes)  # (the device path's lanes too)
                 idx = idx_ctx.filter_batch(text, args.decision_threshold)
                 logger.info("Processing multiallelics -> pre-classifier")
                 sp = split_plans[0] = multiallelics.make_split_plan(
@@ -679,14 +681,15 @@ def run(argv: list[str]):  # noqa: C901, PLR0912, PLR0915
         # copies each contig's blocks verbatim, which needs them to start on a block boundary.
         def device_groups():
             """[[(contig, begin voff, end voff), ...], ...]: pieces adjacent in the file, about group_bytes compressed a group.
-            Contigs longer than that are cut at entries of the tabix linear index (record starts)."""
+            Contigs longer than that are cut at entries of the tabix linear index (record starts).  --treat_multiallelics:
+            one whole contig a group (its overlap clusters must not be cut)."""
             pieces = []
             for c in contigs:
                 if c not in index:
                     continue
                 vb, ve = index[c]
                 cuts = [vb]
-                if not multi:
+                if not multi and not split_device:
                     for v in linear_index.get(c, ()):
                         if (int(v) >> 16) - (cuts[-1] >> 16) >= group_bytes and (ve >> 16) - (int(v) >> 16) >= group_bytes // 4:
                             cuts.append(int(v))
@@ -696,7 +699,7 @@ def run(argv: list[str]):  # noqa: C901, PLR0912, PLR0915
             for c, vb, ve in pieces:
                 span = (ve >> 16) - (vb >> 16)
                 # blacklist positions are uploaded per call for one contig: with blacklists a group holds one contig
-                if cur and (multi or vb != cur[-1][2] or cur_bytes + span > group_bytes + group_bytes // 4 or
+                if cur and (multi or split_device or vb != cur[-1][2] or cur_bytes + span > group_bytes + group_bytes // 4 or
                             (blacklists is not None and c != cur[-1][0])):
                     groups.append(cur)
                     cur, cur_bytes = [], 0
@@ -735,7 +738,8 @@ def run(argv: list[str]):  # noqa: C901, PLR0912, PLR0915
                 got = fh.readinto(memoryview(comp))
             if got != c1 - c0:
                 raise OSError(f"{args.input_file}: short read of {group[0][0]}..{group[-1][0]}")
-            return "device", comp, skip, take, bufs, [g for g, _ in live], np.array(starts, dtype=np.uint64)
+            ref = multiallelics.read_fasta_contig(args.ref_fasta, group[0][0], as_bytes=True) if split_device else None
+            return "device", comp, skip, take, bufs, [g for g, _ in live], np.array(starts, dtype=np.uint64), ref
 
         def load_work(group: list[tuple]):
             return load_group(group) if device_io else load_contig(group[0][0])
@@ -745,8 +749,11 @@ def run(argv: list[str]):  # noqa: C901, PLR0912, PLR0915
         gpu_pool = ThreadPoolExecutor(max_workers=n_lanes, thread_name_prefix="ugvc-device")
         flying: list[tuple] = []
         n_calls = 0
+        # --treat_multiallelics on the device: a split handle per lane (a handle serves one stream at a time)
+        lane_plans = [multiallelics.DeviceSplitPlan(header, header.loader_columns(args.custom_annotations), b"", device)
+                      for _ in range(n_lanes)] if split_device else []
 
-        def device_call(lane: int, comp, skip: int, take: int, in_bufs: dict, starts, bl_pos):
+        def device_call(lane: int, comp, skip: int, take: int, in_bufs: dict, starts, bl_pos, ref):
             ctx.bind_thread()
             n_max = take // 32 + 1024
             # VCF text deflates to well under half its size; text that does not comes back as UGVC_E_FALLBACK
@@ -756,11 +763,20 @@ def run(argv: list[str]):  # noqa: C901, PLR0912, PLR0915
                 sizes["end"] = (n_max, np.int64)
             out_bufs = out_pool.acquire(sizes, grow=max_span / max(1, comp.size))
             try:
-                res = ctx.filter_bgzf_edits(comp, skip, take, args.decision_threshold, file_flags, n_max, with_model=with_model,
-                                            recalibrate_genotype=recal, blacklists=bl_pos, want_end=out.index_info_end,
-                                            lane=lane, bufs={k: v[1] for k, v in out_bufs.items()})
-                first = ctx.filter_bgzf_first_records(starts, lane=lane) if res is not None else None
-                ms = ctx.filter_bgzf_stage_ms(lane) if res is not None else None
+                if split_device:
+                    sp = lane_plans[lane]
+                    sp.set_reference(ref)
+                    res = sp.filter_bgzf(ctx, idx_ctx, comp, skip, take, args.decision_threshold, file_flags, n_max,
+                                         recalibrate_genotype=recal, blacklists=bl_pos, want_end=out.index_info_end, lane=lane,
+                                         bufs={k: v[1] for k, v in out_bufs.items()})
+                    first = np.zeros(1, dtype=np.int64) if res is not None else None
+                    ms = ctx.filter_bgzf_split_stage_ms(lane) if res is not None else None
+                else:
+                    res = ctx.filter_bgzf_edits(comp, skip, take, args.decision_threshold, file_flags, n_max, with_model=with_model,
+                                                recalibrate_genotype=recal, blacklists=bl_pos, want_end=out.index_info_end,
+                                                lane=lane, bufs={k: v[1] for k, v in out_bufs.items()})
+                    first = ctx.filter_bgzf_first_records(starts, lane=lane) if res is not None else None
+                    ms = ctx.filter_bgzf_stage_ms(lane) if res is not None else None
             except BaseException:
                 out_pool.release(out_bufs)
                 raise
@@ -787,10 +803,12 @@ def run(argv: list[str]):  # noqa: C901, PLR0912, PLR0915
                         if again is not None:
                             host_contig(c, again)
                     continue
-                dev_ms += np.array(ms)
+                dev_ms[: len(ms)] += np.array(ms)
                 bounds = np.concatenate((first, [res["n_records"]])).astype(np.int64)
                 for k, (c, _vb, _ve) in enumerate(live):
                     logger.info(f"{int(bounds[k + 1] - bounds[k])} variants found on {c}")
+                if split_device:
+                    logger.info("Processing multiallelics -> pre-classifier")
                 logger.info("Writing records")
                 out.write_device_batch([g[0] for g in live], bounds, res, release=lambda b=out_bufs: out_pool.release(b))
                 totals["n_records"] += res["n_records"]
@@ -819,7 +837,7 @@ def run(argv: list[str]):  # noqa: C901, PLR0912, PLR0915
             if not isinstance(loaded[0], str):
                 host_contig(group[0][0], loaded)
                 continue
-            _tag, comp, skip, take, in_bufs, live, starts = loaded  # ("device", compressed blocks, ...)
+            _tag, comp, skip, take, in_bufs, live, starts, ref = loaded  # ("device", compressed blocks, ...)
             if blacklists is not None:
                 logger.info("Applying blacklist")
             if args.blacklist_cg_insertions:
@@ -834,15 +852,23 @@ def run(argv: list[str]):  # noqa: C901, PLR0912, PLR0915
                 ctx.set_key_order(*lib.learn_key_order(head[: head.rfind(b"\n") + 1]))
                 key_order_set = True
             need = (take + (1 << 17) + 4096, take // 32 + 1024)  # whole blocks are inflated: up to 64 KiB either side of the range
+            # --treat_multiallelics: the index pass reads the contig, the scored pass the kept lines and up to two split rows
+            # for every record taken out (a contig that outgrows this comes back as a fall-back)
+            need_idx, need = (need, (2 * need[0], 2 * need[1])) if split_device else (None, need)
             t_alloc = time.perf_counter()
-            if need[0] > reserved[0] or need[1] > reserved[1]:
+            if need[0] > reserved[0] or need[1] > reserved[1] or \
+                    (need_idx and (need_idx[0] > idx_reserved[0] or need_idx[1] > idx_reserved[1])):
                 drain_device(0)  # the lanes' buffers are about to move
                 ahead = max(1.0, max_span / max(1, comp.size)) * 1.05  # the largest group, at this one's compression ratio
-                reserved = (max(int(need[0] * ahead), reserved[0]), max(int(need[1] * ahead), reserved[1]))
-                ctx.reserve(reserved[0], reserved[1], n_lanes)
+                if need[0] > reserved[0] or need[1] > reserved[1]:
+                    reserved = (max(int(need[0] * ahead), reserved[0]), max(int(need[1] * ahead), reserved[1]))
+                    ctx.reserve(reserved[0], reserved[1], n_lanes)
+                if need_idx and (need_idx[0] > idx_reserved[0] or need_idx[1] > idx_reserved[1]):
+                    idx_reserved = (max(int(need_idx[0] * ahead), idx_reserved[0]), max(int(need_idx[1] * ahead), idx_reserved[1]))
+                    idx_ctx.reserve(idx_reserved[0], idx_reserved[1], n_lanes)
             seconds["alloc"] += time.perf_counter() - t_alloc
             drain_device(n_lanes - 1)  # at most n_lanes calls in flight, each on its own lane and stream
-            flying.append((live, gpu_pool.submit(device_call, n_calls % n_lanes, comp, skip, take, in_bufs, starts, bl_pos)))
+            flying.append((live, gpu_pool.submit(device_call, n_calls % n_lanes, comp, skip, take, in_bufs, starts, bl_pos, ref)))
             n_calls += 1
             if n_calls == 1:
                 drain_device(0)  # the first call alone: every lazy one-time set-up of the path happens on one thread
@@ -876,10 +902,15 @@ def run(argv: list[str]):  # noqa: C901, PLR0912, PLR0915
                     "deflate+write %.2f, index %.2f (+ %.2f at close)", seconds["inflate_wait"], seconds["alloc"], seconds["gpu"],
                     out.seconds["splice"], out.seconds["deflate"], out.seconds.get("index", 0.0), time.perf_counter() - t_close)
         logger.info("start-up seconds: " + ", ".join(f"{k} {v:.2f}" for k, v in startup.items()))
-        if device_io:
+        if split_device:
+            logger.info("device split path, ms on the GPU: H2D + inflate %.0f, index K1 %.0f, split build %.0f, scored K1..K3 %.0f, "
+                        "merge + score %.0f, record writer %.0f, deflate + pack %.0f, D2H %.0f", *dev_ms)
+        elif device_io:
             logger.info("device file path, ms on the GPU: H2D + inflate %.0f, K1..K3 %.0f, record writer %.0f, deflate + pack %.0f, "
-                        "D2H %.0f", *dev_ms)
+                        "D2H %.0f", *dev_ms[:5])
         ctx.close()
+        for sp in lane_plans:
+            sp.close()
         if idx_ctx is not None:
             idx_ctx.close()
         if split_plans[0] is not None and hasattr(split_plans[0], "close"):

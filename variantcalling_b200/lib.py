@@ -132,6 +132,11 @@ SIGNATURES = {
     "ugvc_test_write_records": (C.c_int64, [_vp, _vp, _sz, _vp, _vp, C.c_int64, _vp, _vp, _vp, C.c_int, C.c_int,
                                             C.POINTER(FileEdits), _vp, _sz, _vp]),
     "ugvc_filter_bgzf_stage_ms": (C.c_int, [_vp, C.c_int, _vp]),
+    "ugvc_filter_bgzf_split": (C.c_int, [_vp, _vp, _vp, C.c_int, _vp, _sz, C.c_uint32, C.c_uint64, _vp, _sz, C.c_double, C.c_int,
+                                         C.POINTER(FileEdits), _vp, _sz, C.POINTER(_sz), _vp, _sz, C.POINTER(_sz), _vp, _vp, _vp,
+                                         _sz, C.POINTER(C.c_int64), _vp]),
+    "ugvc_filter_bgzf_split_stage_ms": (C.c_int, [_vp, C.c_int, _vp]),
+    "ugvc_test_ma_score": (C.c_int, [_vp, _vp, C.c_int64, C.c_int, C.c_double, _vp, _vp, _vp]),
     "ugvc_filter_bgzf_first_records": (C.c_int, [_vp, C.c_int, _vp, C.c_int, _vp]),
     "ugvc_test_parse_float": (C.c_int, [C.c_char_p, C.POINTER(C.c_float), C.POINTER(C.c_double),
                                         C.POINTER(C.c_int)]),
@@ -372,6 +377,43 @@ class Context:
                 res["end"] = end[: res["n_records"]]
         return res
 
+    def filter_bgzf_split(self, bgzf: np.ndarray, skip_head: int, take_bytes: int, threshold: float, flags: int,
+                          max_records: int, *, index_ctx: "Context", ma, ref: np.ndarray, split_stats: np.ndarray,
+                          recalibrate_genotype: bool = False, blacklists: list[tuple[str, np.ndarray]] | None = None,
+                          want_end: bool = False, lane: int = 0, bufs: dict | None = None) -> dict | None:
+        """--treat_multiallelics on the file path (see ugvc_filter_bgzf_split): one whole contig, with `index_ctx` (the
+        model-less plan, reserved with this lane) for the index pass, `ma` (a ugvc_ma handle) for the split and `ref` (the
+        contig's sequence, uint8) -- results as :meth:`filter_bgzf_edits`.  Needs enable_phreds(2) before reserve.
+        `split_stats` (int64[8]) receives out_split; the reference's failures come back as UgvcDataError (see
+        multiallelics.DeviceSplitPlan.filter_bgzf, which maps them).  None when the contig needs the host path."""
+        end = None
+        if want_end:
+            end = bufs["end"] if bufs is not None and "end" in bufs else np.empty(max(1, max_records), np.int64)
+        e, keep = _file_edits(True, recalibrate_genotype, blacklists, end)  # noqa: F841  (keep: alive for the call)
+        ref = np.ascontiguousarray(ref, dtype=np.uint8)
+        res = self._filter_bgzf(bgzf, skip_head, take_bytes, threshold, flags, max_records, lane, bufs, e,
+                                split=(index_ctx.h, ma, ref, split_stats))
+        if res is not None:
+            res["n_blacklisted"] = int(e.n_blacklisted)
+            if end is not None:
+                res["end"] = end[: res["n_records"]]
+        return res
+
+    def filter_bgzf_split_stage_ms(self, lane: int = 0) -> list[float]:
+        """ms of the last filter_bgzf_split call on `lane`: H2D + inflate, index K1, split build, scored K1..K3,
+        merge + score, record writer, deflate + pack, D2H."""
+        ms = (C.c_float * 8)()
+        self._check(self.lib.ugvc_filter_bgzf_split_stage_ms(self.h, lane, C.cast(ms, C.c_void_p)))
+        return list(ms)
+
+    def test_ma_score(self, lik: np.ndarray, threshold: float) -> tuple[np.ndarray, np.ndarray, np.ndarray]:
+        """The split path's score kernel on (n, width) likelihoods (test hook ugvc_test_ma_score): phreds, qual, low."""
+        lik = np.ascontiguousarray(lik, dtype=np.float64)
+        n, width = lik.shape
+        ph, q, low = np.empty_like(lik), np.empty(n, np.float64), np.empty(n, np.uint8)
+        self._check(self.lib.ugvc_test_ma_score(self.h, _ptr(lik), n, width, threshold, _ptr(ph), _ptr(q), _ptr(low)))
+        return ph, q, low
+
     def test_write_records(self, text, line_start, recinfo, flags: int, *, low_score=None, qual=None, phreds=None,
                            with_model: bool = True, recalibrate_genotype: bool = False, blacklists=None,
                            want_end: bool = False) -> dict | None:
@@ -400,7 +442,7 @@ class Context:
             res["end"] = end[:n]
         return res
 
-    def _filter_bgzf(self, bgzf, skip_head, take_bytes, threshold, flags, max_records, lane, bufs, edits):
+    def _filter_bgzf(self, bgzf, skip_head, take_bytes, threshold, flags, max_records, lane, bufs, edits, split=None):
         comp = np.ascontiguousarray(bgzf, dtype=np.uint8)
         if bufs is not None:  # the caller's (pinned, reused) buffers: out, blocks, ri, ls, low
             out, blocks, ri, ls, low = bufs["out"], bufs["blocks"], bufs["ri"], bufs["ls"], bufs["low"]
@@ -414,7 +456,12 @@ class Context:
         nb, nblk, n = C.c_size_t(), C.c_size_t(), C.c_int64()
         args = (_ptr(out), out.size, C.byref(nb), _ptr(blocks), blocks.size, C.byref(nblk), _ptr(ri), _ptr(ls), _ptr(low),
                 max_records, C.byref(n))
-        if edits is None:
+        if split is not None:
+            idx_h, ma, ref, stats = split
+            rc = self.lib.ugvc_filter_bgzf_split(self.h, idx_h, ma, lane, _ptr(comp), comp.size, skip_head, take_bytes,
+                                                 _ptr(ref) if ref.size else None, ref.size, threshold, flags, C.byref(edits),
+                                                 *args, _ptr(stats))
+        elif edits is None:
             rc = self.lib.ugvc_filter_bgzf(self.h, lane, _ptr(comp), comp.size, skip_head, take_bytes, threshold, flags, *args)
         else:
             rc = self.lib.ugvc_filter_bgzf_edits(self.h, lane, _ptr(comp), comp.size, skip_head, take_bytes, threshold, flags,

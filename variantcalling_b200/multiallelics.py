@@ -20,7 +20,8 @@ as ordinary records:
   SplitPlan.merge()             ->  N x W likelihood matrix in input record order
 
 ``DeviceSplitPlan`` runs find_overlaps / build / merge as CUDA kernels (csrc/multiallelic.cu, C ABI ``ugvc_ma_*``) and is
-what the tool uses; ``SplitPlan`` is the same algorithm in Python -- the model the kernels were written from, kept for
+what the tool uses -- on the device file path (``DeviceSplitPlan.filter_bgzf``) chained with the inflate, both passes,
+the score math, the record writer and the deflate on device pointers; ``SplitPlan`` is the same algorithm in Python -- the model the kernels were written from, kept for
 differential tests and as ``UGVC_MA_HOST=1`` (A/B), like ``UGVC_K1_LEGACY`` for the generic parser.
 The reference's error behaviour is kept (see DESIGN.md section 4): no multi-allelic site on a
 contig -> ValueError, no deletion cluster -> KeyError('spanning_deletion'), a called genotype
@@ -602,6 +603,7 @@ class DeviceSplitPlan:
 
         self._lib = lib.load_library()
         self._UgvcError = lib.UgvcError
+        self._UgvcDataError = lib.UgvcDataError
         self.host = SplitPlan(header, loaded_columns, "")  # the rule tables only (its build / merge are not used)
         self.set_reference(ref_seq)
         h = C.c_void_p()
@@ -657,23 +659,10 @@ class DeviceSplitPlan:
         rc = self._lib.ugvc_ma_build(self.h, text.ctypes.data, text.size, line_start.ctypes.data, recinfo.ctypes.data, n,
                                      self.ref.ctypes.data if self.ref.size else None, self.ref.size,
                                      self.stats.ctypes.data_as(C.POINTER(C.c_int64)))
-        n_singles, n_cluster = int(self.stats[0]), int(self.stats[1])
         if rc not in (0, -4):
             self._check(rc)
-        err_group, err_code = -1, 0
-        if rc == -4:  # noqa: PLR2004  (UGVC_E_DATA)
-            g, c = C.c_int64(), C.c_int32()
-            self._lib.ugvc_ma_data_error(self.h, C.byref(g), C.byref(c))
-            err_group, err_code = g.value, c.value
-        # the order in which the reference meets its failures (training_prep.py:255-287)
-        if n_singles == 0:
-            raise ValueError("No objects to concatenate")  # pd.concat([]) in training_prep.py:261
-        if 0 <= err_group < n_singles:
-            self._raise(err_code)
-        if n_cluster == 0:
-            raise KeyError("spanning_deletion")  # variant_filtering_utils.py:339 on a frame without the column
-        if err_group >= 0:
-            self._raise(err_code)
+        self._raise_reference_failure()
+        n_singles, n_cluster = int(self.stats[0]), int(self.stats[1])
         n_groups = n_singles + n_cluster
         out = np.empty(int(self.stats[4] + self.stats[5]), dtype=np.uint8)
         self.origins = np.empty(n_groups, dtype=np.int32)
@@ -691,6 +680,42 @@ class DeviceSplitPlan:
         exc, msg = _MA_ERRORS.get(code, (RuntimeError, f"device split failed with code {code}"))
         raise exc(msg)
 
+    def _raise_reference_failure(self, merge_failed: bool = False):
+        """Raise what the reference raises on the contig of the last build (self.stats) or merge, in the order in which it
+        meets its failures (training_prep.py:255-287, then merge_and_assign_pls); nothing when there is none."""
+        n_singles, n_cluster = int(self.stats[0]), int(self.stats[1])
+        err_group, err_code = -1, 0
+        g, c = C.c_int64(-1), C.c_int32(0)
+        if not merge_failed and self._lib.ugvc_ma_data_error(self.h, C.byref(g), C.byref(c)) == 0:
+            err_group, err_code = g.value, c.value
+        if n_singles == 0:
+            raise ValueError("No objects to concatenate")  # pd.concat([]) in training_prep.py:261
+        if 0 <= err_group < n_singles:
+            self._raise(err_code)
+        if n_cluster == 0:
+            raise KeyError("spanning_deletion")  # variant_filtering_utils.py:339 on a frame without the column
+        if err_group >= 0:
+            self._raise(err_code)
+        if merge_failed:
+            raise IndexError("list index out of range")  # a 2-class model has no hom-alt likelihood to spread
+
+    def filter_bgzf(self, ctx, index_ctx, bgzf, skip_head: int, take_bytes: int, threshold: float, flags: int,
+                    max_records: int, **kw) -> dict | None:
+        """One whole contig through the device file path with this plan's handle and reference
+        (``lib.Context.filter_bgzf_split``; ``kw`` as there).  The reference's failures keep their types, as in
+        ``build`` / ``merge``; the result also holds "split_stats" (``ugvc_ma_build``'s counts)."""
+        try:
+            res = ctx.filter_bgzf_split(bgzf, skip_head, take_bytes, threshold, flags, max_records, index_ctx=index_ctx,
+                                        ma=self.h, ref=self.ref, split_stats=self.stats, **kw)
+        except self._UgvcDataError:
+            if self.stats[7] == 0:  # a data error of K1, not of the split
+                raise
+            self._raise_reference_failure(merge_failed=self.stats[7] == 2)  # noqa: PLR2004
+            raise
+        if res is not None:
+            res["split_stats"] = self.stats.copy()
+        return res
+
     def merge(self, lik: np.ndarray) -> np.ndarray:
         """``SplitPlan.merge``: (n_kept + n_split, K) likelihoods -> (N, W) in input record order."""
         lik = np.ascontiguousarray(lik, dtype=np.float64)
@@ -700,8 +725,8 @@ class DeviceSplitPlan:
         width = max(k, int(self.stats[6]))
         out = np.empty((int(self.kept.size), width), dtype=np.float64)
         rc = self._lib.ugvc_ma_merge(self.h, lik.ctypes.data, n_rows, k, out.ctypes.data, width)
-        if rc == -4:  # noqa: PLR2004
-            raise IndexError("list index out of range")  # a 2-class model has no hom-alt likelihood to spread
+        if rc == -4:  # noqa: PLR2004  (UGVC_E_DATA)
+            self._raise_reference_failure(merge_failed=True)
         self._check(rc)
         return out
 
