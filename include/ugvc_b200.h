@@ -480,11 +480,12 @@ int ugvc_test_device_deflate(ugvc_ctx* ctx, const uint8_t* data, size_t n, int e
 int ugvc_test_device_inflate(ugvc_ctx* ctx, const uint8_t* bgzf, size_t n_bytes, int decoder, uint8_t* out, size_t capacity,
                              size_t* out_n, int32_t* block_rc, size_t block_capacity, size_t* out_n_blocks);
 /* Test hook: the K3 launch the loaded plan gets (also in the host emulation, which runs the same chunking).
- * out = {kernel (0 k3_heap, 1 k3_infer), threads per CTA, tile buffers per group, groups per CTA (records per tile:
- * threads / groups), trees one thread walks at once, forest chunk (k3_heap: trees, k3_infer: nodes; 0 for a linear
- * model), 1 when the whole model is staged once, CTAs of the persistent grid, tree walk (0 plain; 1 default-left /
- * categorical routing of an xgboost model with such nodes)}.  UGVC_E_STATE without a model. */
-int ugvc_test_k3_config(ugvc_ctx* ctx, int32_t out[9]);
+ * out = {kernel (0 k3_heap, 1 k3_infer), threads per CTA, tile buffers per group, groups per CTA, trees one thread
+ * walks at once, forest chunk (k3_heap: trees, k3_infer: nodes; 0 for a linear model), 1 when the whole model is staged
+ * once, CTAs of the persistent grid, tree walk (0 plain; 1 default-left / categorical routing of an xgboost model with
+ * such nodes), threads per record (2: k3_heap_split)}.  Records per tile: threads / groups / threads per record.
+ * UGVC_E_STATE without a model. */
+int ugvc_test_k3_config(ugvc_ctx* ctx, int32_t out[10]);
 int ugvc_test_parse_float(const char* text, float* out_f32, double* out_f64, int* out_consumed);
 /* Test hook: the device BGZF encoder (csrc/deflate.cuh) run on the host on one block of at most 57344 bytes (4 readable
  * bytes after n); out receives a complete BGZF block (<= 65536 bytes), the size is returned. */

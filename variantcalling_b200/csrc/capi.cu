@@ -158,6 +158,7 @@ static void free_lane(Lane& l) {
     cudaFree(l.b.slow_list);
     cudaFree(l.b.line_start);
     cudaFree(l.b.n_records);
+    cudaFree(l.b.k3_ticket);
     cudaFree(l.b.raw);
     cudaFree(l.b.recinfo);
     cudaFree(l.b.feats);
@@ -872,6 +873,7 @@ extern "C" int ugvc_reserve(ugvc_ctx* ctx, size_t max_bytes, size_t max_records,
         CU(cudaMalloc(&l.b.slow_list, max_records * sizeof(uint32_t)));
         CU(cudaMalloc(&l.b.line_start, (max_records + 1) * sizeof(int64_t)));
         CU(cudaMalloc(&l.b.n_records, sizeof(int64_t)));
+        CU(cudaMalloc(&l.b.k3_ticket, sizeof(unsigned)));
         CU(cudaMalloc(&l.b.raw, (size_t)p.h.n_slots * max_records * sizeof(uint32_t)));
         CU(cudaMalloc(&l.b.recinfo, max_records * sizeof(ugvc_recinfo)));
         CU(cudaMalloc(&l.b.feats, (size_t)p.h.n_features * max_records * sizeof(float)));
@@ -920,7 +922,7 @@ static int enqueue_kernels(ugvc_ctx* ctx, Lane& l, const uint8_t* d_text, size_t
     if (timing) CU(cudaEventRecord(ev[3], st));
     if (has_model)
         launch_k3(p, ctx->k3, l.b.raw, l.b.feats, l.b.cap_records, d_n_records, threshold, d_low, d_probs, d_qual,
-                  d_low == l.b.low_score ? l.b.phreds : nullptr, ctx->want_phreds, ctx->d_counts, l.d_err, st);
+                  d_low == l.b.low_score ? l.b.phreds : nullptr, ctx->want_phreds, ctx->d_counts, l.d_err, l.b.k3_ticket, st);
     if (timing) CU(cudaEventRecord(ev[4], st));
     ctx->launches += (has_model ? (fused ? 1 : 2) : 0) + (fast ? 2 : 2 + (p.h.n_slots ? 1 : 0));
     CU(cudaGetLastError());
@@ -1988,7 +1990,7 @@ extern "C" int ugvc_predict_features(ugvc_ctx* ctx, const float* x, size_t n, si
     const int64_t n64 = (int64_t)n;
     CU(cudaMemcpyAsync(l.b.n_records, &n64, sizeof(n64), cudaMemcpyHostToDevice, st));
     launch_k3(p, ctx->k3, nullptr, l.b.feats, l.b.cap_records, l.b.n_records, threshold, l.b.low_score, l.b.probs, l.b.qual,
-              l.b.phreds, ctx->want_phreds, ctx->d_counts, l.d_err, st);
+              l.b.phreds, ctx->want_phreds, ctx->d_counts, l.d_err, l.b.k3_ticket, st);
     ctx->launches += 1;
     CU(cudaGetLastError());
     if (out_low_score) CU(cudaMemcpyAsync(out_low_score, l.b.low_score, n, cudaMemcpyDeviceToHost, st));
@@ -2136,13 +2138,13 @@ extern "C" int ugvc_test_device_sigmoid(ugvc_ctx*, const float*, int, float*, fl
 extern "C" int ugvc_test_format_g(ugvc_ctx*, const float*, int64_t, uint8_t*) { return UGVC_E_CUDA; }
 #endif
 
-extern "C" int ugvc_test_k3_config(ugvc_ctx* ctx, int32_t out[9]) {
+extern "C" int ugvc_test_k3_config(ugvc_ctx* ctx, int32_t out[10]) {
     // test hook: the K3 launch the loaded plan gets
     if (!ctx || !out) return UGVC_E_ARG;
     if (!ctx->has_plan || ctx->plan.h.model_kind == MODEL_NONE)
         return fail(ctx, UGVC_E_STATE, "test_k3_config: load a plan with a model first");
     const K3Config& c = ctx->k3;
-    const int32_t v[9] = {c.kernel, c.tpb, c.nbuf, c.groups, c.nch, (int32_t)c.chunk, c.resident ? 1 : 0, c.grid, c.walk};
+    const int32_t v[10] = {c.kernel, c.tpb, c.nbuf, c.groups, c.nch, (int32_t)c.chunk, c.resident ? 1 : 0, c.grid, c.walk, c.split};
     memcpy(out, v, sizeof(v));
     return UGVC_OK;
 }

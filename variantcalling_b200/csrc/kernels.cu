@@ -1385,6 +1385,51 @@ __device__ __forceinline__ void walkhc(const uint8_t* __restrict__ s_node, const
     for (int j = 0; j < NCH; ++j) leaf[j] = (int)s_leaf[(a8[j] >> 3) - H];
 }
 
+// The leaf rows of trees [tr, min(tr + NCH, c1)) into the accumulators, in tree order (the sums both k3_heap forms
+// share).  Binary sklearn boosting keeps the leaf values of a group pending (fetched from global memory, L1) while the
+// next group is walked, and adds them before it: k3_add_pending adds what is left after the last group.
+template <int NCH>
+__device__ __forceinline__ void k3_add_pending(double z[UGVC_MAX_CLASSES], const double pend[NCH], unsigned n_pend) {
+#pragma unroll
+    for (int j = 0; j < NCH; ++j)
+        if ((unsigned)j < n_pend) z[0] = __dadd_rn(z[0], pend[j]);
+}
+template <int NCH>
+__device__ __forceinline__ void k3_add_leaves(const DevPlan& plan, unsigned tr, unsigned c1, const int leaf[NCH],
+                                              double z[UGVC_MAX_CLASSES], float zf[UGVC_MAX_CLASSES], double pend[NCH],
+                                              unsigned& n_pend) {
+    const int K = plan.h.n_classes, O = plan.h.n_outputs;
+    if (plan.h.model_kind == MODEL_GB_SKLEARN && O == 1) {
+        // raw += learning_rate * leaf (pre-scaled on the host), fp64, tree order
+        k3_add_pending<NCH>(z, pend, n_pend);
+        n_pend = c1 - tr < (unsigned)NCH ? c1 - tr : (unsigned)NCH;
+#pragma unroll
+        for (int j = 0; j < NCH; ++j) pend[j] = __ldg(&plan.leaves[leaf[j]]);
+    } else if (plan.h.model_kind == MODEL_RF_SKLEARN) {
+#pragma unroll
+        for (int j = 0; j < NCH; ++j)
+            if (tr + j < c1) {
+                const double* lv = plan.leaves + (size_t)leaf[j] * plan.h.leaf_width;
+#pragma unroll
+                for (int k = 0; k < UGVC_MAX_CLASSES; ++k)
+                    if (k < K) z[k] = __dadd_rn(z[k], __ldg(&lv[k]));
+            }
+    } else {
+#pragma unroll
+        for (int j = 0; j < NCH; ++j)
+            if (tr + j < c1) {
+                const int o = plan.tree_out[tr + j];
+                const double add = __ldg(&plan.leaves[leaf[j]]);
+                const float addf = (float)add;
+#pragma unroll
+                for (int k = 0; k < UGVC_MAX_CLASSES; ++k) {
+                    z[k] = o == k ? __dadd_rn(z[k], add) : z[k];
+                    zf[k] = o == k ? __fadd_rn(zf[k], addf) : zf[k];
+                }
+            }
+    }
+}
+
 // NBUF = 2: the raw rows of the NEXT record tile are fetched by 1-D bulk copies (cp.async.bulk, one per feature row,
 // completion on an mbarrier) while the current tile is walked, so no warp ever waits on HBM; every thread then turns
 // its own column of the landed slot words into feature values in place (K2's policies) -- a thread only ever reads
@@ -1395,9 +1440,9 @@ __global__ void __launch_bounds__(TPB, 1)
 k3_heap(const __grid_constant__ DevPlan plan, const uint32_t* __restrict__ raw, const float* __restrict__ feats,
         size_t row_stride, const int64_t* __restrict__ n_records_p, double threshold, uint8_t* __restrict__ low_score,
         float* __restrict__ probs, double* __restrict__ qual_out, double* __restrict__ phred_out, long long* counts,
-        unsigned chunk_trees, int phred_mode, unsigned long long* err) {
+        unsigned chunk_trees, int phred_mode, unsigned long long* err, unsigned*) {
     extern __shared__ __align__(16) uint8_t smem3[];
-    const int F = plan.h.n_features, K = plan.h.n_classes, O = plan.h.n_outputs;
+    const int F = plan.h.n_features;
     const unsigned n_trees = plan.h.n_trees;
     const bool forest = plan.h.model_kind != MODEL_LOGISTIC;
     const int depth = (int)plan.heap_depth;
@@ -1559,41 +1604,9 @@ k3_heap(const __grid_constant__ DevPlan plan, const uint32_t* __restrict__ raw, 
                     if (WALK == K3_WALK_CAT) walkhc<NCH>(reinterpret_cast<const uint8_t*>(s_node), s_leaf, s_cat, H, depth, lt, lt_end, xcol, leaf);
                     else if (plan.h.cmp_mode == CMP_LE) walkh<CMP_LE, NCH>(reinterpret_cast<const uint8_t*>(s_node), s_leaf, H, depth, lt, lt_end, xcol, leaf);
                     else walkh<CMP_LT, NCH>(reinterpret_cast<const uint8_t*>(s_node), s_leaf, H, depth, lt, lt_end, xcol, leaf);
-                    if (plan.h.model_kind == MODEL_GB_SKLEARN && O == 1) {
-                        // raw += learning_rate * leaf (pre-scaled on the host), fp64, tree order
-#pragma unroll
-                        for (int j = 0; j < NCH; ++j)
-                            if ((unsigned)j < n_pend) z[0] = __dadd_rn(z[0], pend[j]);
-                        n_pend = c1 - tr < (unsigned)NCH ? c1 - tr : (unsigned)NCH;
-#pragma unroll
-                        for (int j = 0; j < NCH; ++j) pend[j] = __ldg(&plan.leaves[leaf[j]]);
-                    } else if (plan.h.model_kind == MODEL_RF_SKLEARN) {
-#pragma unroll
-                        for (int j = 0; j < NCH; ++j)
-                            if (tr + j < c1) {
-                                const double* lv = plan.leaves + (size_t)leaf[j] * plan.h.leaf_width;
-#pragma unroll
-                                for (int k = 0; k < UGVC_MAX_CLASSES; ++k)
-                                    if (k < K) z[k] = __dadd_rn(z[k], __ldg(&lv[k]));
-                            }
-                    } else {
-#pragma unroll
-                        for (int j = 0; j < NCH; ++j)
-                            if (tr + j < c1) {
-                                const int o = plan.tree_out[tr + j];
-                                const double add = __ldg(&plan.leaves[leaf[j]]);
-                                const float addf = (float)add;
-#pragma unroll
-                                for (int k = 0; k < UGVC_MAX_CLASSES; ++k) {
-                                    z[k] = o == k ? __dadd_rn(z[k], add) : z[k];
-                                    zf[k] = o == k ? __fadd_rn(zf[k], addf) : zf[k];
-                                }
-                            }
-                    }
+                    k3_add_leaves<NCH>(plan, tr, c1, leaf, z, zf, pend, n_pend);
                 }
-#pragma unroll
-                for (int j = 0; j < NCH; ++j)
-                    if ((unsigned)j < n_pend) z[0] = __dadd_rn(z[0], pend[j]);
+                k3_add_pending<NCH>(z, pend, n_pend);
                 c0 = c1;
             }
         }
@@ -1620,18 +1633,261 @@ k3_heap(const __grid_constant__ DevPlan plan, const uint32_t* __restrict__ raw, 
     }
 }
 
+// k3_heap with two threads per record (resident forests only).  Thread A of a record walks trees [0, TA), thread B
+// walks [TA, T) and leaves its leaf rows in s_hand; A then adds them after its own, so the record's sums are the same
+// roundings in the same tree order as k3_heap's (z = init + l0 + ... + l(T-1)).  For the same feature tile the CTA
+// runs twice the warps and twice the walk chains.  The CTA is GROUPS independent groups (own tile, own mbarrier, named
+// barrier), each of RS = TPB / GROUPS / 2 records: threads [0, RS) of a group are the A threads, [RS, 2 RS) the B
+// threads, so every warp reads 32 distinct tile columns.  A group claims its tiles from the launch's ticket (zeroed
+// by launch_k3), so the groups that finish first take the last tiles; the first warp of a group claims, then spreads
+// the tile's row copies over its lanes.  NBUF = 2: the group's next tile is claimed and in flight while it walks the
+// current one.  In the host emulation (one thread, RS = 1) that thread plays B, then A, through the same code.
+__host__ __device__ inline unsigned k3s_trees_a(unsigned n_trees, unsigned nch) {  // TA: half the trees, whole groups of chains
+    const unsigned a = ((n_trees + 1) / 2 + nch - 1) / nch * nch;
+    return a < n_trees ? a : n_trees;
+}
+template <int TPB, int NBUF, int NCH, int GROUPS, int WALK = K3_WALK_PLAIN>
+__global__ void __launch_bounds__(TPB, 1)
+k3_heap_split(const __grid_constant__ DevPlan plan, const uint32_t* __restrict__ raw, const float* __restrict__ feats,
+              size_t row_stride, const int64_t* __restrict__ n_records_p, double threshold, uint8_t* __restrict__ low_score,
+              float* __restrict__ probs, double* __restrict__ qual_out, double* __restrict__ phred_out, long long* counts,
+              unsigned, int phred_mode, unsigned long long* err, unsigned* __restrict__ ticket) {
+    // NBUF = 2 (one group of 192 records, 384 threads, the next tile in flight during the walk) measured 1.35 ms per
+    // bench launch against 0.96 ms for five single-buffered groups of 64 (profiles/h100_k3_budget.json): the warps
+    // the second buffer costs outweigh the fetch it hides.  The buffer index is kept so that it can be timed again.
+    static_assert(NBUF == 1 || NBUF == 2, "one or two tile buffers per group");
+    extern __shared__ __align__(16) uint8_t smem3[];
+    const int F = plan.h.n_features;
+    const unsigned n_trees = plan.h.n_trees, ta = k3s_trees_a(n_trees, NCH), tb = n_trees - ta;
+    const int depth = (int)plan.heap_depth;
+    const unsigned H = 1u << depth;
+    constexpr int GS = TPB / GROUPS;  // threads of one group
+    constexpr int RS = GS / 2;        // records of one group's tile
+    const int gid = GROUPS == 1 ? 0 : (int)threadIdx.x / GS, gtid = GROUPS == 1 ? (int)threadIdx.x : (int)threadIdx.x % GS;
+    const int r = gtid % RS;
+    float* tile0 = reinterpret_cast<float*>(smem3) + (size_t)gid * NBUF * F * RS;                               // [NBUF][F][RS]
+    uint2* s_node = reinterpret_cast<uint2*>(reinterpret_cast<float*>(smem3) + (size_t)GROUPS * NBUF * F * RS);  // [T][H]
+    PlanFeature* s_pf = reinterpret_cast<PlanFeature*>(s_node + (size_t)n_trees * H);                      // [F]
+    uint16_t* s_leaf = reinterpret_cast<uint16_t*>(s_pf + F);                                              // [T][H]
+    uint16_t* s_hand0 = s_leaf + (size_t)n_trees * H;                                                      // [GROUPS][tb][RS]
+    uint32_t* s_cat = reinterpret_cast<uint32_t*>(s_hand0 + (size_t)GROUPS * tb * RS);                     // [n_cat_words]
+    uint16_t* s_hand = s_hand0 + (size_t)gid * tb * RS;
+    for (int i = threadIdx.x; i < F; i += blockDim.x) s_pf[i] = plan.feats[i];
+    if (WALK == K3_WALK_CAT) {
+        const uint32_t* cat = reinterpret_cast<const uint32_t*>(plan.dev_nodes + plan.h.n_nodes);
+        for (unsigned i = threadIdx.x; i < plan.n_cat_words; i += blockDim.x) s_cat[i] = cat[i];
+    }
+    const uint8_t* heap_flags = plan.heap_feat + (size_t)n_trees * H;  // K3_WALK_CAT: the node flags follow the features
+    // (stride blockDim.x: TPB threads on the device, one in the host emulation)
+    for (unsigned i = threadIdx.x; i < n_trees * H; i += blockDim.x) {
+        const unsigned fl = WALK == K3_WALK_CAT ? (unsigned)heap_flags[i] << 30 : 0u;
+        s_node[i] = make_uint2(__float_as_uint(plan.heap_thr[i]), (unsigned)plan.heap_feat[i] * (unsigned)(RS * sizeof(float)) | fl);
+        s_leaf[i] = plan.heap_leaf[i];
+    }
+    const long long n_rec = *n_records_p;
+    const long long n_tiles = (n_rec + RS - 1) / RS;
+    const int fa = (F + 1) / 2;  // K2: A assembles features [0, fa), B [fa, F)
+    unsigned n_low = 0, n_seen = 0;
+#ifdef UGVC_HOST_EMU
+    constexpr int ROLES = 2;  // the one thread is B, then A
+#else
+    constexpr int ROLES = 1;
+    __shared__ __align__(8) unsigned long long k3_mbar_all[GROUPS * NBUF];
+    __shared__ unsigned s_tile_all[GROUPS * NBUF];  // the tile claimed into each buffer
+    unsigned long long* k3_mbar = k3_mbar_all + gid * NBUF;
+    unsigned* s_tile = s_tile_all + gid * NBUF;
+    if (threadIdx.x == 0) {
+        for (int b = 0; b < GROUPS * NBUF; ++b)
+            asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"((uint32_t)__cvta_generic_to_shared(&k3_mbar_all[b])));
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+    // the group's first warp: claim the next tile for buffer b, then its rows [t * RS, ...) of every feature's slot ->
+    // buffer b.  Past the last tile only the arrival completes the buffer's phase, and the group reads that it is done.
+    auto claim_fetch = [&](int b) {
+        const int lane = gtid;
+        const uint32_t mb = (uint32_t)__cvta_generic_to_shared(&k3_mbar[b]);
+        if (lane == 0) s_tile[b] = atomicAdd(ticket, 1u);
+        __syncwarp();
+        const long long t = s_tile[b];
+        if (t >= n_tiles) {
+            if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(mb) : "memory");
+            return;
+        }
+        float* tile = tile0 + (size_t)b * F * RS;
+        const size_t rec0 = (size_t)t * RS;
+        const size_t rows = row_stride - rec0 < (size_t)RS ? row_stride - rec0 : (size_t)RS;  // rows are padded to 128 records
+        const uint32_t row_bytes = (uint32_t)rows * 4u;
+        if (lane == 0)
+            asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(mb), "r"(row_bytes * (uint32_t)F) : "memory");
+        __syncwarp();
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+        for (int f = lane; f < F; f += 32) {
+            const void* src = raw ? static_cast<const void*>(raw + (size_t)s_pf[f].slot * row_stride + rec0)
+                                  : static_cast<const void*>(feats + (size_t)f * row_stride + rec0);
+            const uint32_t dst = (uint32_t)__cvta_generic_to_shared(tile + (size_t)f * RS);
+            asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                         ::"r"(dst), "l"(src), "r"(row_bytes), "r"(mb)
+                         : "memory");
+        }
+    };
+    uint32_t phases = 0u;  // bit b: the parity buffer b waits for next
+    if (gtid < 32)
+        for (int b = 0; b < NBUF; ++b) claim_fetch(b);
+#endif
+    auto group_sync = [&]() {
+#ifndef UGVC_HOST_EMU
+        if (GROUPS == 1) __syncthreads();
+        else asm volatile("bar.sync %0, %1;" ::"r"(gid + 1), "r"(GS) : "memory");
+#endif
+    };
+    for (int buf = 0;; buf = NBUF == 2 ? buf ^ 1 : 0) {
+#ifdef UGVC_HOST_EMU
+        const long long t = atomicAdd(ticket, 1u);
+#else
+        {
+            const uint32_t mb = (uint32_t)__cvta_generic_to_shared(&k3_mbar[buf]);
+            uint32_t ok = 0;
+            while (!ok)
+                asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
+                             : "=r"(ok)
+                             : "r"(mb), "r"((phases >> buf) & 1u)
+                             : "memory");
+            phases ^= 1u << buf;
+        }
+        const long long t = s_tile[buf];
+#endif
+        if (t >= n_tiles) break;
+        float* tile = tile0 + (size_t)buf * F * RS;
+        const long long rec = t * RS + r;
+        const bool active = rec < n_rec;
+        // K2 (transformers.py:221-344): each thread of the pair assembles its half of the record's features; a combine
+        // runs in the thread that assembled its feature, after it
+        for (int role = 0; role < ROLES; ++role) {
+            const int half = ROLES == 2 ? 1 - role : gtid / RS;
+            const int f0 = half ? fa : 0, f1 = half ? F : fa;
+            if (raw) {
+                const uint32_t* src = raw + rec;
+#pragma unroll 2
+                for (int f = f0; f < f1; ++f) {
+                    const PlanFeature pf = s_pf[f];
+#ifdef UGVC_HOST_EMU
+                    const uint32_t bits = active ? src[(size_t)pf.slot * row_stride] : 0u;
+#else
+                    const uint32_t bits = __float_as_uint(tile[f * RS + r]);
+#endif
+                    tile[f * RS + r] = active ? k2_apply(bits, pf, rec, f, err) : 0.f;
+                }
+                for (unsigned c = 0; c < plan.h.n_combines; ++c) {  // feature = max(feature, slot_b), nulls skipped
+                    const PlanCombine cb = plan.combines[c];
+                    if (active && (int)cb.feature >= f0 && (int)cb.feature < f1)
+                        k2_combine_one(cb, __ldg(src + (size_t)cb.slot_b * row_stride), tile[cb.feature * RS + r], rec, true, err);
+                }
+                for (unsigned c = 0; c < plan.h.n_checks && half == 0; ++c) {
+                    const PlanCheck ck = plan.checks[c];
+                    if (!active) continue;
+                    const uint32_t bits = __ldg(src + (size_t)ck.slot * row_stride);
+                    if (bits == RAW_ABSENT || bits == RAW_MISSING) continue;  // handled by the feature policies
+                    const float v = __uint_as_float(bits);
+                    const bool ok = ck.kind == 0 ? (v <= ck.bound) : (v >= ck.bound);
+                    if (!ok) atomicMin(err, ugvc_pack_error(rec, 0xFFFF, ck.kind == 0 ? REASON_TOO_MANY_ELEMS : REASON_BAD_VALUE));
+                }
+            } else {
+#ifdef UGVC_HOST_EMU
+                const float* src = feats + rec;
+                for (int f = f0; f < f1; ++f) tile[f * RS + r] = active ? src[(size_t)f * row_stride] : 0.f;
+#else
+                if (!active)
+                    for (int f = f0; f < f1; ++f) tile[f * RS + r] = 0.f;
+#endif
+            }
+        }
+        group_sync();  // the pair's features are in the tile
+        const uint8_t* xcol = reinterpret_cast<const uint8_t*>(tile + r);
+        const uint8_t* nodes = reinterpret_cast<const uint8_t*>(s_node);
+        double z[UGVC_MAX_CLASSES];   // fp64 accumulators (sklearn) ...
+        float zf[UGVC_MAX_CLASSES];   // ... fp32 accumulators (xgboost), A's only
+        double pend[NCH];
+        unsigned n_pend = 0;
+        for (int role = 0; role < ROLES; ++role) {
+            const int half = ROLES == 2 ? 1 - role : gtid / RS;
+            if (half == 0) {
+#pragma unroll
+                for (int o = 0; o < UGVC_MAX_CLASSES; ++o) {
+                    z[o] = plan.h.model_kind == MODEL_RF_SKLEARN ? 0.0 : plan.h.init[o];
+                    zf[o] = (float)plan.h.init[o];
+                }
+            }
+            const unsigned t0 = half ? ta : 0, t1 = half ? n_trees : ta;
+            for (unsigned tr = t0; tr < t1; tr += NCH) {
+                int leaf[NCH];
+                if (WALK == K3_WALK_CAT) walkhc<NCH>(nodes, s_leaf, s_cat, H, depth, tr, t1, xcol, leaf);
+                else if (plan.h.cmp_mode == CMP_LE) walkh<CMP_LE, NCH>(nodes, s_leaf, H, depth, tr, t1, xcol, leaf);
+                else walkh<CMP_LT, NCH>(nodes, s_leaf, H, depth, tr, t1, xcol, leaf);
+                if (half) {  // B: hand the leaf rows over, one row of s_hand per tree
+#pragma unroll
+                    for (int j = 0; j < NCH; ++j)
+                        if (tr + j < t1) s_hand[(size_t)(tr - ta + j) * RS + r] = (uint16_t)leaf[j];
+                } else {
+                    k3_add_leaves<NCH>(plan, tr, t1, leaf, z, zf, pend, n_pend);
+                }
+            }
+        }
+        group_sync();  // B's leaf rows are in s_hand, and the walks are done with the tile
+#ifndef UGVC_HOST_EMU
+        // k3_finish reads the tile only for a linear model: this buffer takes a new tile while A finishes this one.  B
+        // writes s_hand again only after the next tile's first barrier, which A reaches after reading it.
+        if (gtid < 32) claim_fetch(buf);
+#endif
+        if (ROLES == 2 || gtid < RS) {
+            // A: B's trees, in tree order after its own
+            for (unsigned tr = ta; tr < n_trees; tr += NCH) {
+                int leaf[NCH];
+#pragma unroll
+                for (int j = 0; j < NCH; ++j) leaf[j] = tr + j < n_trees ? (int)s_hand[(size_t)(tr - ta + j) * RS + r] : 0;
+                k3_add_leaves<NCH>(plan, tr, n_trees, leaf, z, zf, pend, n_pend);
+            }
+            k3_add_pending<NCH>(z, pend, n_pend);
+            if (active) {
+                const bool low = k3_finish<RS>(plan, reinterpret_cast<const float*>(xcol), z, zf, rec, threshold, low_score,
+                                               probs, qual_out, phred_out, phred_mode);
+                n_low += low ? 1u : 0u;
+                n_seen += 1u;
+            }
+        }
+    }
+#pragma unroll
+    for (int s = 16; s > 0; s >>= 1) {
+        n_low += __shfl_xor_sync(0xffffffffu, n_low, s);
+        n_seen += __shfl_xor_sync(0xffffffffu, n_seen, s);
+    }
+    if ((threadIdx.x & 31) == 0 && n_seen) {
+        atomicAdd((unsigned long long*)&counts[0], (unsigned long long)n_seen);
+        atomicAdd((unsigned long long*)&counts[1], (unsigned long long)n_low);
+        atomicAdd((unsigned long long*)&counts[2], (unsigned long long)(n_seen - n_low));
+    }
+}
+
 // ------------------------------------------------------------------------------------------
 // The K3 launch of a plan: kernel, shape, staging, grid and walk (k3_choose, once per plan)
 // ------------------------------------------------------------------------------------------
-// k3_heap's instantiations {tpb, nbuf, nch, groups}, records per tile tpb / groups.  Entries 0-7 are tried in order
-// (UGVC_K3_SHAPE picks one of them): two half-CTAs with one tile each first (most warps for the shared memory), then
-// double-buffered single groups.  Where there are few threads per SM (the tiles are large), sixteen trees per thread
-// in flight make up for it.  Entry 8 is entry 1 walking twelve trees at once (UGVC_K3_NCH448=12).
+// k3_heap's instantiations {tpb, nbuf, nch, groups, split}, records per tile tpb / groups / split.  Entry 9
+// (k3_heap_split: five groups of 64 records, two threads per record, 20 warps) comes first for a resident forest of
+// K3S_MIN_TREES trees or more, at most K3S_MAX_DEPTH deep, that it holds and entry 0 does not; five groups keep four other tiles walking while one
+// waits for its rows.  Then entries 0-7 are tried in order (UGVC_K3_SHAPE picks one of 0-7 or 9): two half-CTAs with
+// one tile each first (most warps for the shared memory), then double-buffered single groups.  Where there are few
+// threads per SM (the tiles are large), sixteen trees per thread in flight make up for it.  Entry 8 is entry 1 walking
+// twelve trees at once (UGVC_K3_NCH448=12).
 struct K3hShape {
-    int tpb, nbuf, nch, groups;
+    int tpb, nbuf, nch, groups, split = 1;
 };
 static constexpr K3hShape K3H_SHAPES[] = {{512, 1, 8, 2},  {448, 1, 8, 2}, {384, 1, 16, 2}, {256, 2, 16, 1}, {192, 2, 16, 1},
-                                          {128, 2, 16, 1}, {256, 1, 8, 1}, {128, 1, 8, 1},  {448, 1, 12, 2}};
+                                          {128, 2, 16, 1}, {256, 1, 8, 1}, {128, 1, 8, 1},  {448, 1, 12, 2}, {640, 1, 8, 5, 2}};
+static constexpr int K3S_SHAPE = 9;
+// k3_heap_split needs trees to share: with fewer, each thread of a pair walks at most four groups of chains and the
+// two extra barriers and the hand-over of every tile weigh more (UGVC_K3_SHAPE=9 runs it on any forest it holds)
+static constexpr unsigned K3S_MIN_TREES = 64;
+static constexpr unsigned K3S_MAX_DEPTH = 6;
 // k3_infer's instantiations: records per CTA, 384 when the feature tile and the whole forest still fit, else 256
 static constexpr int K3I_TPB[] = {384, 256};
 
@@ -1642,12 +1898,24 @@ static size_t k3h_tile_bytes(const DevPlan& plan, K3hShape c) {  // all tile buf
     return (size_t)c.nbuf * plan.h.n_features * c.tpb * sizeof(float) + (size_t)plan.h.n_features * sizeof(PlanFeature) + 64 +
            k3_cat_bytes(plan);
 }
+// k3_heap_split's shared memory: the groups' tiles, the policy table, bitsets, the whole forest and the hand-over rows
+static size_t k3s_bytes(const DevPlan& plan, K3hShape c) {
+    const size_t rs = (size_t)c.tpb / c.groups / 2, tb = plan.h.n_trees - k3s_trees_a(plan.h.n_trees, (unsigned)c.nch);
+    return (size_t)c.groups * c.nbuf * plan.h.n_features * rs * sizeof(float) + (size_t)plan.h.n_features * sizeof(PlanFeature) + 64 +
+           k3_cat_bytes(plan) + (size_t)plan.h.n_trees * k3h_tree_bytes(plan) + (size_t)c.groups * tb * rs * sizeof(uint16_t);
+}
 // the K3H_SHAPES entry of a model with a heap form, -1 if none holds it
 static int k3h_shape(const DevPlan& plan) {
-    static const int force = getenv("UGVC_K3_SHAPE") ? atoi(getenv("UGVC_K3_SHAPE")) : -1;  // profiling knob: index 0-7
+    static const int force = getenv("UGVC_K3_SHAPE") ? atoi(getenv("UGVC_K3_SHAPE")) : -1;  // profiling knob: 0-7 or 9
     static const int nch448 = getenv("UGVC_K3_NCH448") ? atoi(getenv("UGVC_K3_NCH448")) : 8;  // profiling knob
     const bool forest = plan.h.model_kind != MODEL_LOGISTIC;
     const size_t all = forest ? (size_t)plan.h.n_trees * k3h_tree_bytes(plan) : 0;
+    // k3_heap_split where the tile leaves the one-thread form short of its widest shape (16 warps), for forests of the
+    // depth it was timed at (the bench's, 6) or shallower; deeper ones keep k3_heap until a measurement says otherwise
+    const bool split_pays = force < 0 && plan.h.n_trees >= K3S_MIN_TREES && plan.heap_depth <= K3S_MAX_DEPTH &&
+                            k3h_tile_bytes(plan, K3H_SHAPES[0]) + all > K3_SMEM_BUDGET;
+    if (forest && (force == K3S_SHAPE || split_pays) && k3s_bytes(plan, K3H_SHAPES[K3S_SHAPE]) <= K3_SMEM_BUDGET)
+        return K3S_SHAPE;
     for (int i = 0; i < 8; ++i) {
         if (force >= 0 && i != force) continue;
         if (k3h_tile_bytes(plan, K3H_SHAPES[i]) + all <= K3_SMEM_BUDGET) return i == 1 && nch448 == 12 ? 8 : i;
@@ -1675,11 +1943,13 @@ static K3Config k3_heap_config(const DevPlan& plan, int sm_count) {
     c.nbuf = sh.nbuf;
     c.groups = sh.groups;
     c.nch = sh.nch;
-    c.chunk = k3h_chunk_trees(plan, sh);
+    c.split = sh.split;
+    c.chunk = sh.split == 2 ? plan.h.n_trees : k3h_chunk_trees(plan, sh);
     c.resident = plan.h.model_kind == MODEL_LOGISTIC || c.chunk >= plan.h.n_trees;
-    c.smem = k3h_tile_bytes(plan, sh) + (size_t)c.chunk * k3h_tree_bytes(plan);
+    c.smem = sh.split == 2 ? k3s_bytes(plan, sh) : k3h_tile_bytes(plan, sh) + (size_t)c.chunk * k3h_tree_bytes(plan);
     int per_sm = (int)((227u * 1024u) / (c.smem + 1024));
     per_sm = per_sm < 1 ? 1 : (per_sm > 4 ? 4 : per_sm);
+    if (sh.split == 2) per_sm = 1;  // __launch_bounds__(tpb, 1) registers: a second CTA would not be resident
     if (per_sm * sh.tpb > 1536) per_sm = 1536 / sh.tpb;
     c.grid = sm_count * per_sm;
     c.walk = (int)plan.walk;
@@ -1730,7 +2000,7 @@ static K3Config k3_infer_config(const DevPlan& plan, int sm_count) {
     c.kernel = K3_KERNEL_INFER;
     c.shape = k3i_shape(plan);
     c.tpb = K3I_TPB[c.shape];
-    c.nbuf = c.groups = 1;
+    c.nbuf = c.groups = c.split = 1;
     c.nch = K3_CHAINS;
     c.chunk = k3_chunk_nodes(plan);
     c.resident = k3_forest_bytes(plan) == 0 || c.chunk >= plan.h.n_nodes;
@@ -1777,9 +2047,15 @@ bool k3_choose(const DevPlan& plan, const uint32_t* tree_root, int sm_count, K3C
 
 #ifndef UGVC_HOST_EMU
 // the instantiations of one walk, in table order
+template <size_t S, int WALK>
+static constexpr auto k3h_kernel() {
+    constexpr K3hShape sh = K3H_SHAPES[S];
+    if constexpr (sh.split == 2) return &k3_heap_split<sh.tpb, sh.nbuf, sh.nch, sh.groups, WALK>;
+    else return &k3_heap<sh.tpb, sh.nbuf, sh.nch, sh.groups, WALK>;
+}
 template <int WALK, size_t... S>
 static auto k3h_kernels(std::index_sequence<S...>) {
-    return std::array{&k3_heap<K3H_SHAPES[S].tpb, K3H_SHAPES[S].nbuf, K3H_SHAPES[S].nch, K3H_SHAPES[S].groups, WALK>...};
+    return std::array{k3h_kernel<S, WALK>()...};
 }
 template <int WALK, size_t... S>
 static auto k3i_kernels(std::index_sequence<S...>) {
@@ -1793,11 +2069,13 @@ static const auto K3I_KERNELS = std::array{k3i_kernels<K3_WALK_PLAIN>(std::make_
 
 void launch_k3(const DevPlan& plan, const K3Config& c, const uint32_t* raw, const float* feats, size_t row_stride,
                const int64_t* d_n_records, double threshold, uint8_t* low_score, float* probs, double* qual,
-               double* phreds, int phred_mode, long long* d_counts, unsigned long long* d_err, cudaStream_t st) {
+               double* phreds, int phred_mode, long long* d_counts, unsigned long long* d_err, unsigned* ticket,
+               cudaStream_t st) {
     if (c.kernel == K3_KERNEL_HEAP) {
+        if (c.split == 2) cudaMemsetAsync(ticket, 0, sizeof(unsigned), st);
         const auto k = K3H_KERNELS[c.walk][c.shape];
         k<<<c.grid, c.tpb, c.smem, st>>>(plan, raw, feats, row_stride, d_n_records, threshold, low_score, probs, qual, phreds,
-                                         d_counts, c.chunk, phred_mode, d_err);
+                                         d_counts, c.chunk, phred_mode, d_err, ticket);
     } else {
         const auto k = K3I_KERNELS[c.walk][c.shape];
         k<<<c.grid, c.tpb, c.smem, st>>>(plan, feats, row_stride, d_n_records, threshold, low_score, probs, qual, phreds,
@@ -1832,7 +2110,8 @@ cudaError_t kernels_configure(const DevPlan& plan) {
 // forest larger than it runs the chunk loop here too.  smem3 is the emulation's shared memory.
 void launch_k3(const DevPlan& plan, const K3Config& c, const uint32_t* raw, const float* feats, size_t row_stride,
                const int64_t* d_n_records, double threshold, uint8_t* low_score, float* probs, double* qual,
-               double* phreds, int phred_mode, long long* d_counts, unsigned long long* d_err, cudaStream_t) {
+               double* phreds, int phred_mode, long long* d_counts, unsigned long long* d_err, unsigned* ticket,
+               cudaStream_t) {
     threadIdx = blockIdx = dim3(0, 0, 0);
     blockDim = gridDim = dim3(1, 1, 1);
     if (c.smem > sizeof(smem3)) {  // c.smem is sized for the product's tile, wider than the emulated one
@@ -1840,10 +2119,16 @@ void launch_k3(const DevPlan& plan, const K3Config& c, const uint32_t* raw, cons
         abort();
     }
     const bool cat = c.walk == K3_WALK_CAT;
-    if (c.kernel == K3_KERNEL_HEAP)
+    if (c.kernel == K3_KERNEL_HEAP && c.split == 2) {  // one thread: RS = 1 record per tile, walked as B then A
+        *ticket = 0;
+        (cat ? k3_heap_split<2, 1, 8, 1, K3_WALK_CAT> : k3_heap_split<2, 1, 8, 1, K3_WALK_PLAIN>)(
+            plan, raw, feats, row_stride, d_n_records, threshold, low_score, probs, qual, phreds, d_counts, c.chunk,
+            phred_mode, d_err, ticket);
+    }
+    else if (c.kernel == K3_KERNEL_HEAP)
         (cat ? k3_heap<1, 1, 8, 1, K3_WALK_CAT> : k3_heap<1, 1, 8, 1, K3_WALK_PLAIN>)(
             plan, raw, feats, row_stride, d_n_records, threshold, low_score, probs, qual, phreds, d_counts, c.chunk,
-            phred_mode, d_err);
+            phred_mode, d_err, ticket);
     else
         (cat ? k3_infer<1, K3_WALK_CAT> : k3_infer<1, K3_WALK_PLAIN>)(
             plan, feats, row_stride, d_n_records, threshold, low_score, probs, qual, phreds, d_counts, c.chunk, phred_mode);

@@ -154,6 +154,7 @@ struct LaneBuffers {
     uint32_t* slow_list;       // [cap_records] records handed to the generic parser
     int64_t* line_start;       // [cap_records + 1]
     int64_t* n_records;        // device scalar
+    unsigned* k3_ticket;       // device scalar: k3_heap_split's tile ticket
     // K1
     uint32_t* raw;             // [n_slots][cap_records]
     ugvc_recinfo* recinfo;     // [cap_records]
@@ -189,7 +190,8 @@ enum { K3_KERNEL_HEAP = 0, K3_KERNEL_INFER = 1 };
 struct K3Config {
     int kernel;             // K3_KERNEL_HEAP / K3_KERNEL_INFER
     int shape;              // the kernel's instantiation: index into kernels.cu's K3H_SHAPES / K3I_TPB
-    int tpb, nbuf, groups;  // threads per CTA, tile buffers per group, independent groups per CTA (records per tile: tpb / groups)
+    int tpb, nbuf, groups;  // threads per CTA, tile buffers per group, independent groups per CTA
+    int split;              // threads per record (k3_heap_split: 2; records per tile: tpb / groups / split)
     int nch;                // trees one thread walks at once
     unsigned chunk;         // k3_heap: trees per staged forest chunk; k3_infer: nodes the forest buffer holds (0: linear model)
     bool resident;          // the whole model is staged once (no chunk loop)
@@ -204,6 +206,7 @@ bool k3_choose(const DevPlan& plan, const uint32_t* tree_root, int sm_count, K3C
 // K3 as c says.  k3_heap reads the raw slots, or the dense feature matrix feats when raw is NULL; k3_infer reads feats.
 void launch_k3(const DevPlan& plan, const K3Config& c, const uint32_t* raw, const float* feats, size_t row_stride,
                const int64_t* d_n_records, double threshold, uint8_t* low_score, float* probs, double* qual,
-               double* phreds, int phred_mode, long long* d_counts, unsigned long long* d_err, cudaStream_t st);
+               double* phreds, int phred_mode, long long* d_counts, unsigned long long* d_err, unsigned* ticket,
+               cudaStream_t st);
 size_t k1_smem_bytes(const DevPlan& plan);
 cudaError_t kernels_configure(const DevPlan& plan);

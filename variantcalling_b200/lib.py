@@ -554,11 +554,12 @@ class Context:
 
     def k3_config(self) -> dict:
         """The K3 launch the loaded plan gets (test hook ugvc_test_k3_config)."""
-        out = np.zeros(9, np.int32)
+        out = np.zeros(10, np.int32)
         self._check(self.lib.ugvc_test_k3_config(self.h, _ptr(out)))
-        kernel, tpb, nbuf, groups, nch, chunk, resident, grid, walk = (int(v) for v in out)
+        kernel, tpb, nbuf, groups, nch, chunk, resident, grid, walk, split = (int(v) for v in out)
         return {"kernel": ("heap", "infer")[kernel], "tpb": tpb, "nbuf": nbuf, "groups": groups, "nch": nch, "chunk": chunk,
-                "resident": bool(resident), "grid": grid, "gs": tpb // groups, "walk": ("plain", "categorical")[walk]}
+                "resident": bool(resident), "grid": grid, "gs": tpb // groups // split, "split": split,
+                "walk": ("plain", "categorical")[walk]}
 
     def test_format_g(self, values) -> np.ndarray:
         """The record writer's "%g" on the device (test hook ugvc_test_format_g): an (n, 16) uint8 array, text in
