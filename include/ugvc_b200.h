@@ -390,6 +390,30 @@ int ugvc_conc_classify(ugvc_conc* h, int64_t n, const int8_t* gt_ultima, const i
                        uint8_t* out_classify, uint8_t* out_classify_gt);
 int ugvc_conc_curve(ugvc_conc* h, int group, double* precision, double* recall, double* thresholds,
                     size_t capacity);
+/* Annotation of a concordance frame (comparison_utils.annotate_concordance, ugbio_comparison/comparison_utils.py:
+ * 321-380; DESIGN.md 4b).  Contigs are uploaded once and stay on the handle: ugvc_conc_annot_add_contig copies one
+ * contig's raw FASTA bytes (case kept) and returns its id; ugvc_conc_annot_clear drops them all.
+ * ugvc_conc_annotate: per record the contig id (-1 = not in the FASTA), 1-based pos, indel (0/1), REF as bytes at
+ * ref_bytes[ref_off[i] .. ref_off[i+1]), and the alleles k in [rec_allele_off[i], rec_allele_off[i+1]) at
+ * allele_bytes[allele_off[k] .. allele_off[k+1]) (every record has at least one allele).  flow_order is a NUL-terminated
+ * string, or NULL for no cycle-skip column.  Outputs, per record: class (0 None, 1 ins, 2 del), indel length, hmer indel
+ * length and base (0 = None), the upper-cased motifs (motif_size bytes per record, zero-padded, lengths apart), the GC fraction
+ * (fp64) and the cycle-skip code (0 NA, 1 cycle-skip, 2 possible-cycle-skip, 3 non-skip).  Where the reference raises,
+ * the call returns UGVC_E_DATA and ugvc_conc_annot_error gives the record it raises at and a UGVC_ANNOT_E_* reason. */
+#define UGVC_ANNOT_E_INDEX 1          /* IndexError: an insertion whose alleles all equal REF */
+#define UGVC_ANNOT_E_KEY 2            /* KeyError: the record's contig is not in the FASTA */
+#define UGVC_ANNOT_E_ZERO_DIVISION 3  /* ZeroDivisionError: an empty GC window */
+int ugvc_conc_annot_add_contig(ugvc_conc* h, const uint8_t* seq, int64_t len, int32_t* out_id);
+int ugvc_conc_annot_clear(ugvc_conc* h);
+int ugvc_conc_annotate(ugvc_conc* h, int64_t n, const int32_t* contig, const int64_t* pos, const uint8_t* indel,
+                       const uint8_t* ref_bytes, const int64_t* ref_off, const uint8_t* allele_bytes,
+                       const int64_t* allele_off, const int64_t* rec_allele_off, const char* flow_order, int motif_size,
+                       int gc_window, int8_t* out_class, int32_t* out_indel_len, int32_t* out_hmer_len,
+                       uint8_t* out_hmer_nuc, uint8_t* out_left, uint8_t* out_right, uint8_t* out_left_len,
+                       uint8_t* out_right_len, double* out_gc, int8_t* out_cycleskip);
+int ugvc_conc_annot_error(const ugvc_conc* h, int64_t* row, int* reason);
+/* CUDA-event time in ms of the kernel of the last ugvc_conc_annotate call (uploads and downloads excluded). */
+double ugvc_conc_annot_kernel_ms(const ugvc_conc* h);
 
 /* ---- --treat_multiallelics on the device (SURVEY.md 8 row f2) -------------
  * Replaces, per contig, the frame surgery of training_prep.process_multiallelic_spandel

@@ -9,17 +9,22 @@ raises.
       -> concordance_utils.py:11-106
   calc_recall_precision_curve(...)                 -> :109-188
   get_concordance_metrics(predictions, scores, truth, fn_mask, ...)   -> :346-458
+  annotate_concordance(concordance_df, fasta, ...)  -> ugbio_comparison/comparison_utils.py:321-380 (the per-record
+      passes in ``csrc/conc_annotate.cu``; interval and filter columns in NumPy / pandas)
 """
 from __future__ import annotations
 
 import ctypes as C
+import itertools
 import logging
+import os
 from collections import OrderedDict
 
 import numpy as np
 import pandas as pd
 
 from variantcalling_b200 import lib
+from variantcalling_b200.multiallelics import read_fasta_contig
 
 logger = logging.getLogger(__name__)
 
@@ -153,6 +158,83 @@ class ConcordanceContext:
         if rc != 0:
             raise lib.UgvcError(rc, self.lib.ugvc_conc_last_error(self.h).decode())
         return tuple(a[:n] for a in out)
+
+
+    def annot_contig(self, fasta: str, contig: str) -> int:
+        """Id of `contig` of `fasta` on the handle (-1 when the FASTA lacks it), read and uploaded on first use."""
+        lib.load_annotation()
+        key = (os.path.abspath(fasta), contig)
+        cache = self.__dict__.setdefault("_annot_contigs", {})
+        if key not in cache:
+            try:
+                seq = read_fasta_contig(fasta, contig, as_bytes=True)
+            except KeyError:
+                cache[key] = -1
+                return -1
+            buf = np.frombuffer(seq, dtype=np.uint8) if seq else np.zeros(1, np.uint8)
+            cid = C.c_int32()
+            rc = self.lib.ugvc_conc_annot_add_contig(self.h, lib._ptr(buf), len(seq), C.byref(cid))  # noqa: SLF001
+            if rc != 0:
+                raise lib.UgvcError(rc, self.lib.ugvc_conc_last_error(self.h).decode())
+            cache[key] = int(cid.value)
+        return cache[key]
+
+    def annotate(self, contig_ids, pos, indel, refs, alleles, flow_order: str | None, motif_size: int = 5,
+                 gc_window: int = 10) -> dict:
+        """The per-record columns of annotate_concordance as typed arrays (see ugvc_conc_annotate).  refs: sequence of
+        str, alleles: sequence of tuples of str, ASCII.  Raises what the reference raises, at the same record."""
+        lib.load_annotation()
+        n = len(refs)
+        contig_ids = np.ascontiguousarray(contig_ids, dtype=np.int32)
+        pos = np.ascontiguousarray(pos, dtype=np.int64)
+        indel = np.ascontiguousarray(indel, dtype=np.uint8)
+        n_alleles = np.fromiter(map(len, alleles), dtype=np.int64, count=n)
+        empty = np.flatnonzero(n_alleles == 0)
+        if len(empty):  # max() of no alleles: classify_indel's indel rows fail first, then indel_length's
+            bad = np.flatnonzero((n_alleles == 0) & (indel != 0))
+            row = int(bad[0] if len(bad) else empty[0])
+            raise ValueError(f"record {row}: max() iterable argument is empty (a record without alleles)")
+        ref_bytes, ref_off = _pack_strings(refs)
+        flat = list(itertools.chain.from_iterable(alleles))
+        al_bytes, al_off = _pack_strings(flat)
+        rec_off = np.zeros(n + 1, dtype=np.int64)
+        np.cumsum(n_alleles, out=rec_off[1:])
+        out = {"class": np.empty(n, np.int8), "indel_length": np.empty(n, np.int32), "hmer_length": np.empty(n, np.int32),
+               "hmer_nuc": np.empty(n, np.uint8), "left": np.zeros((n, motif_size), np.uint8),
+               "right": np.zeros((n, motif_size), np.uint8), "left_len": np.empty(n, np.uint8),
+               "right_len": np.empty(n, np.uint8), "gc": np.empty(n, np.float64),
+               "cycleskip": np.empty(n, np.int8) if flow_order is not None else None}
+        p = lib._ptr  # noqa: SLF001
+        fo = None if flow_order is None else flow_order.encode("ascii")
+        rc = self.lib.ugvc_conc_annotate(self.h, n, p(contig_ids), p(pos), p(indel), p(ref_bytes), p(ref_off),
+                                         p(al_bytes), p(al_off), p(rec_off), fo, motif_size, gc_window, p(out["class"]),
+                                         p(out["indel_length"]), p(out["hmer_length"]), p(out["hmer_nuc"]), p(out["left"]),
+                                         p(out["right"]), p(out["left_len"]), p(out["right_len"]), p(out["gc"]),
+                                         p(out["cycleskip"]))
+        if rc == lib.UGVC_E_DATA:
+            row, reason = C.c_int64(), C.c_int()
+            self.lib.ugvc_conc_annot_error(self.h, C.byref(row), C.byref(reason))
+            raise AnnotationDataError(int(row.value), int(reason.value))
+        if rc != 0:
+            raise lib.UgvcError(rc, self.lib.ugvc_conc_last_error(self.h).decode())
+        return out
+
+
+class AnnotationDataError(Exception):
+    """A record where the reference's annotate_concordance raises: `row` and the UGVC_ANNOT_E_* `reason`."""
+
+    def __init__(self, row: int, reason: int):
+        super().__init__(row, reason)
+        self.row, self.reason = row, reason
+
+
+def _pack_strings(strs) -> tuple[np.ndarray, np.ndarray]:
+    """Sequence of ASCII str -> (bytes as uint8, int64 offsets of len + 1)."""
+    lens = np.fromiter(map(len, strs), dtype=np.int64, count=len(strs))
+    data = "".join(strs).encode("ascii")
+    off = np.zeros(len(strs) + 1, dtype=np.int64)
+    np.cumsum(lens, out=off[1:])
+    return (np.frombuffer(data, dtype=np.uint8) if data else np.zeros(1, np.uint8)), off
 
 
 _default_ctx: ConcordanceContext | None = None
@@ -289,3 +371,107 @@ def calc_recall_precision_curve(concordance_df: pd.DataFrame, classify_column_na
         rows.append({"group": name, "precision": c["precision"], "recall": c["recall"], "f1": c["f1"],
                      "threshold": c["threshold"], "predictions": c["predictions"]})
     return pd.DataFrame(rows, columns=["group", "precision", "recall", "f1", "threshold", "predictions"])
+
+
+# ------------------------------------------------------------------ annotate_concordance (comparison_utils.py:321-380)
+ANNOT_MOTIF_SIZE, ANNOT_GC_WINDOW = 5, 10
+_INDEL_CLASS = np.array([None, "ins", "del"], dtype=object)
+_CYCLE_SKIP = np.array(["NA", "cycle-skip", "possible-cycle-skip", "non-skip"], dtype=object)
+_HMER_NUC = np.array([None] + [chr(b) for b in range(1, 256)], dtype=object)
+
+
+def _object_column(values: np.ndarray, index) -> pd.Series:
+    return pd.Series(values, index=index, dtype=object)
+
+
+def _motif_strings(buf: np.ndarray) -> np.ndarray:
+    """(n, size) zero-padded upper-case motif bytes -> object array of str."""
+    if buf.shape[1] == 0:
+        return np.full(buf.shape[0], "", dtype=object)
+    return np.ascontiguousarray(buf).view(f"S{buf.shape[1]}").ravel().astype(f"U{buf.shape[1]}").astype(object)
+
+
+def _raise_like_the_reference(err: AnnotationDataError, chrom: np.ndarray):
+    """The exception the reference raises at err.row (chained to err, which carries the row)."""
+    row = err.row
+    if err.reason == 1:
+        raise IndexError(f"record {row}: list index out of range (an insertion whose alleles all equal ref)") from err
+    if err.reason == 2:  # noqa: PLR2004
+        raise KeyError(chrom[row]) from err
+    if err.reason == 3:  # noqa: PLR2004
+        raise ZeroDivisionError(f"record {row}: float division by zero (empty GC window)") from err
+    raise RuntimeError(f"record {row}: annotation error {err.reason}") from err
+
+
+def fill_filter_column(df: pd.DataFrame) -> pd.DataFrame:
+    """variant_annotation.py:593-612: missing and empty FILTER values become PASS.  A column created here (or one of
+    NaN only) turns into an object column, as the reference's pandas does when it stores a string in a float column."""
+    if "filter" not in df.columns:
+        df["filter"] = np.nan
+    fill = pd.isna(df["filter"]) | (df["filter"] == "")
+    if fill.any() and df["filter"].dtype.kind == "f":
+        df["filter"] = df["filter"].astype(object)
+    df.loc[fill, "filter"] = "PASS"
+    return df
+
+
+def _annotate_intervals(df: pd.DataFrame, annotfile: str) -> tuple[pd.DataFrame, str]:
+    """variant_annotation.py:549-590: a boolean column named after the BED file, True where a record's pos falls in an
+    interval.  The intervals are sorted by (chromosome, start) only and both NumPy searches run on that order, as in
+    the reference, so overlapping intervals give the reference's answer rather than an exact containment test."""
+    annot = annotfile.split("/")[-1]
+    if annot.endswith(".bed"):
+        annot = annot[:-4]
+    df[annot] = False
+    bed = pd.read_csv(annotfile, names=["chromosome", "start", "end"], usecols=[0, 1, 2], index_col=None, sep="\t")
+    bed = bed.sort_values(["chromosome", "start"])
+    bed["chromosome"] = bed["chromosome"].astype("string")
+    bed_rows = bed.groupby("chromosome").groups
+    for chrom, rows in df.groupby("chrom").groups.items():
+        if chrom not in bed_rows:
+            continue
+        pos = np.array(df.loc[rows, "pos"])
+        after_start = np.searchsorted(np.array(bed.loc[bed_rows[chrom], "start"]), pos) - 1
+        before_end = np.searchsorted(np.array(bed.loc[bed_rows[chrom], "end"]), pos)
+        df.loc[rows, annot] = after_start == before_end
+    return df, annot
+
+
+def annotate_concordance(concordance_df: pd.DataFrame, fasta: str, bw_high_quality: list[str] | None = None,
+                         bw_all_quality: list[str] | None = None, annotate_intervals: list[str] | None = None,
+                         flow_order: str | None = "TGCA", ctx: ConcordanceContext | None = None,
+                         ) -> tuple[pd.DataFrame, list]:
+    """comparison_utils.py:321-380.  Adds, in the reference's order, indel_classify, indel_length, hmer_indel_length,
+    hmer_indel_nuc, left_motif, right_motif, gc_content (one kernel launch over all records), one boolean column per
+    interval file, fills `filter`, and adds cycleskip_status when flow_order is not None.  The frame is changed in place
+    and returned with the list of interval column names.  Coverage from bigWig files is not supported."""
+    interval_files = [] if annotate_intervals is None else annotate_intervals
+    if bw_all_quality is not None and bw_high_quality is not None:
+        raise NotImplementedError("coverage from bigWig files (get_coverage) is not supported")
+    df = concordance_df
+    ctx = _context(ctx)
+    codes, names = pd.factorize(df["chrom"], use_na_sentinel=False)
+    ids = np.array([ctx.annot_contig(fasta, str(c)) for c in names], dtype=np.int32)
+    chrom = np.asarray(names, dtype=object)[codes]
+    try:
+        res = ctx.annotate(ids[codes] if len(ids) else np.zeros(0, np.int32), df["pos"].to_numpy(dtype=np.int64),
+                           df["indel"].to_numpy(dtype=bool), df["ref"].tolist(), df["alleles"].tolist(), flow_order,
+                           ANNOT_MOTIF_SIZE, ANNOT_GC_WINDOW)
+    except AnnotationDataError as e:
+        _raise_like_the_reference(e, chrom)
+    idx = df.index
+    df["indel_classify"] = _object_column(_INDEL_CLASS[res["class"]], idx)
+    df["indel_length"] = res["indel_length"].astype(np.int64)
+    df["hmer_indel_length"] = res["hmer_length"].astype(np.int64)
+    df["hmer_indel_nuc"] = _object_column(_HMER_NUC[res["hmer_nuc"]], idx)
+    df["left_motif"] = _object_column(_motif_strings(res["left"]), idx)
+    df["right_motif"] = _object_column(_motif_strings(res["right"]), idx)
+    df["gc_content"] = res["gc"]
+    annots = []
+    for path in interval_files:
+        df, annot = _annotate_intervals(df, path)
+        annots.append(annot)
+    df = fill_filter_column(df)
+    if flow_order is not None:
+        df["cycleskip_status"] = _object_column(_CYCLE_SKIP[res["cycleskip"]], idx)
+    return df, annots

@@ -21,41 +21,10 @@
 //   C4 conc_curve      precision = tps / (tps + fps), recall = tps / tps[-1] in fp64 (IEEE division, the
 //                      same bits as NumPy), written in increasing-threshold order like sklearn returns them
 #include <cub/cub.cuh>
-#include <cuda_runtime.h>
-#include <stdint.h>
 
-#include <string>
-#include <vector>
+#include <algorithm>
 
-#include "../../include/ugvc_b200.h"
-
-#define CONC_GROUPS UGVC_CONC_GROUPS      // 7 default groups + INDELS + H-INDELS
-#define CONC_COUNTERS UGVC_CONC_COUNTERS  // tp, fp, missed (call < truth), initial_tp, n_called, n_fn
-#define CONC_TPB 256
-
-struct ugvc_conc {
-    int device = 0;
-    int sm_count = 132;  // replaced by the device's count when the handle opens
-    cudaStream_t st = nullptr;
-    std::string err;
-    long long launches = 0;
-    double* curve[CONC_GROUPS][3] = {};  // precision, recall, threshold
-    int64_t curve_len[CONC_GROUPS] = {};
-};
-
-static thread_local std::string g_conc_err;
-
-static int conc_fail(ugvc_conc* h, int code, const std::string& msg) {
-    if (h) h->err = msg;
-    g_conc_err = msg;
-    return code;
-}
-#define CCU(call)                                                                                   \
-    do {                                                                                            \
-        cudaError_t e_ = (call);                                                                    \
-        if (e_ != cudaSuccess)                                                                      \
-            return conc_fail(h, UGVC_E_CUDA, std::string(#call) + ": " + cudaGetErrorString(e_)); \
-    } while (0)
+#include "concordance.cuh"
 
 // meta bits: 0-3 default group + 1 (0 = none), 4 truth, 5 false negative, 6 call, 7 indel, 8 hmer > 0
 __device__ __forceinline__ bool conc_member(unsigned meta, int g) {
@@ -153,45 +122,6 @@ __global__ void __launch_bounds__(CONC_TPB) conc_curve(int64_t d, int64_t n_sel,
 struct U8ToI64 {
     __host__ __device__ __forceinline__ int64_t operator()(const uint8_t& v) const { return (int64_t)v; }
 };
-
-extern "C" int ugvc_conc_create(int device, ugvc_conc** out) {
-    ugvc_conc* h = nullptr;
-    if (!out) return conc_fail(nullptr, UGVC_E_ARG, "conc_create: out is NULL");
-    int n_dev = 0;
-    if (cudaGetDeviceCount(&n_dev) != cudaSuccess || n_dev <= 0)
-        return conc_fail(nullptr, UGVC_E_CUDA, "conc_create: no CUDA device (there is no CPU path)");
-    if (device < 0 || device >= n_dev) return conc_fail(nullptr, UGVC_E_ARG, "conc_create: device out of range");
-    h = new ugvc_conc();
-    h->device = device;
-    if (cudaSetDevice(device) != cudaSuccess || cudaStreamCreate(&h->st) != cudaSuccess) {
-        delete h;
-        return conc_fail(nullptr, UGVC_E_CUDA, "conc_create: cannot create a stream");
-    }
-    cudaDeviceGetAttribute(&h->sm_count, cudaDevAttrMultiProcessorCount, device);
-    *out = h;
-    return UGVC_OK;
-}
-
-static void conc_drop_curves(ugvc_conc* h) {
-    for (int g = 0; g < CONC_GROUPS; ++g) {
-        for (int a = 0; a < 3; ++a) {
-            if (h->curve[g][a]) cudaFree(h->curve[g][a]);
-            h->curve[g][a] = nullptr;
-        }
-        h->curve_len[g] = 0;
-    }
-}
-
-extern "C" void ugvc_conc_free(ugvc_conc* h) {
-    if (!h) return;
-    cudaSetDevice(h->device);
-    conc_drop_curves(h);
-    if (h->st) cudaStreamDestroy(h->st);
-    delete h;
-}
-
-extern "C" const char* ugvc_conc_last_error(const ugvc_conc* h) { return h ? h->err.c_str() : g_conc_err.c_str(); }
-extern "C" long long ugvc_conc_launch_count(const ugvc_conc* h) { return h ? h->launches : 0; }
 
 namespace {
 struct DevBuf {  // frees on scope exit

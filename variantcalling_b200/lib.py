@@ -105,6 +105,12 @@ SIGNATURES = {
     "ugvc_conc_run": (C.c_int, [_vp, C.c_int64, _vp, _vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int, _vp, _vp, _vp, _vp]),
     "ugvc_conc_classify": (C.c_int, [_vp, C.c_int64, _vp, _vp, _vp, _vp, _vp]),
     "ugvc_conc_curve": (C.c_int, [_vp, C.c_int, _vp, _vp, _vp, _sz]),
+    "ugvc_conc_annot_add_contig": (C.c_int, [_vp, _vp, C.c_int64, _vp]),
+    "ugvc_conc_annot_clear": (C.c_int, [_vp]),
+    "ugvc_conc_annotate": (C.c_int, [_vp, C.c_int64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, C.c_char_p, C.c_int,
+                                     C.c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "ugvc_conc_annot_error": (C.c_int, [_vp, _vp, _vp]),
+    "ugvc_conc_annot_kernel_ms": (C.c_double, [_vp]),
     "ugvc_ma_create": (C.c_int, [C.c_int, C.POINTER(_vp)]),
     "ugvc_ma_free": (None, [_vp]),
     "ugvc_ma_last_error": (C.c_char_p, [_vp]),
@@ -142,7 +148,12 @@ SIGNATURES = {
                                         C.POINTER(C.c_int)]),
 }
 
+# the concordance-frame annotation entry points are bound on first use (load_annotation), so that a build of the
+# library without them, such as the host emulation of the filter path, still loads
+_BOUND_ON_USE = frozenset(n for n in SIGNATURES if n.startswith("ugvc_conc_annot"))
+
 _lib = None
+_annotation_bound = False
 
 
 def load_library() -> C.CDLL:
@@ -155,11 +166,27 @@ def load_library() -> C.CDLL:
                 f"(make -C variantcalling_b200/csrc).  There is no CPU fallback for the hot path.")
         lib = C.CDLL(LIB_PATH)
         for name, (res, args) in SIGNATURES.items():
+            if name in _BOUND_ON_USE:
+                continue
             fn = getattr(lib, name)
             fn.restype = res
             fn.argtypes = args
         _lib = lib
     return _lib
+
+
+def load_annotation() -> C.CDLL:
+    """load_library() with the annotation entry points bound.  Raises if the library lacks them."""
+    global _annotation_bound  # noqa: PLW0603
+    lib = load_library()
+    if not _annotation_bound:
+        for name in sorted(_BOUND_ON_USE):
+            res, args = SIGNATURES[name]
+            fn = getattr(lib, name)
+            fn.restype = res
+            fn.argtypes = args
+        _annotation_bound = True
+    return lib
 
 
 def _ptr(a):
