@@ -480,6 +480,57 @@ int ugvc_filter_bgzf_split_stage_ms(ugvc_ctx* ctx, int lane, float out_ms[8]);
 int ugvc_test_ma_score(ugvc_ctx* ctx, const double* lik, int64_t n, int width, double threshold, double* out_phreds,
                        double* out_qual, uint8_t* out_low);
 
+/* ---- filter_low_af_ratio_to_background on the device (DESIGN.md 4c) -------
+ * Replaces ugbio_filtering/filter_low_af_ratio_to_background.py:35-65 and process_record (:75-114): per record, unless
+ * FILTER holds RefCall, the AF-ratio rule over every sample (GT / VAF / BG_VAF typed by the header as pysam does) and the
+ * FILTER edit of pysam's record.filter.clear() / add() (htslib bcf_add_filter): new_filter is removed from the list, and
+ * added back when the rule fails the record.  Every byte outside FILTER is kept as read.
+ *   variant_type_kind  1: INFO/VARIANT_TYPE is declared Number=1 String/Character (compared with "h-indel"); 0: never equal
+ *   vaf_kind / bg_vaf_kind  UGVC_AFR_KIND_*; *_integer: Type=Integer (else Float) */
+#define UGVC_AFR_KIND_NONE 0    /* absent from the header: the value is None */
+#define UGVC_AFR_KIND_SCALAR 1  /* Number=1: a scalar, whose len() raises TypeError */
+#define UGVC_AFR_KIND_TUPLE 2   /* any other Number */
+#define UGVC_AFR_MAX_FILTER_BYTES 63
+#define UGVC_AFR_E_LITERAL 1    /* a GT / VAF / BG_VAF literal the parser refuses (numparse.h) */
+#define UGVC_AFR_E_TYPE 2       /* TypeError: len() of a Number=1 VAF / BG_VAF */
+#define UGVC_AFR_FAILED 1
+#define UGVC_AFR_REWRITTEN 2
+#define UGVC_AFR_NEW_CONTIG 4
+typedef struct ugvc_afr_params {
+    double af_ratio_threshold;
+    double af_ratio_threshold_h_indels;
+    double t_vaf_threshold;
+    const char* new_filter;  /* 1..UGVC_AFR_MAX_FILTER_BYTES bytes, not NUL-terminated */
+    int32_t new_filter_len;
+    int32_t variant_type_kind;
+    int32_t vaf_kind, vaf_integer;
+    int32_t bg_vaf_kind, bg_vaf_integer;
+} ugvc_afr_params;
+/* One range of whole VCF data lines per call, in the shape of ugvc_filter_bgzf: `data` = consecutive BGZF blocks
+ * (skip_head / take_bytes as there) or, with is_text != 0, the plain text itself (skip_head must be 0).  The text is
+ * inflated on the device, indexed by K1 of the context's plan (load the model-less plan), decided, written with its new
+ * FILTER column and BGZF-compressed there; outputs as ugvc_filter_bgzf: out_bgzf (blocks of 57344 uncompressed bytes),
+ * out_block_csize, out_line_start (n + 1 entries, offsets in this call's output), out_recinfo (POS, len(REF) in
+ * flags >> 8), plus out_end (INFO/END of each record, 0 where none; may be NULL), out_flags (may be NULL; per record
+ * UGVC_AFR_FAILED | UGVC_AFR_REWRITTEN | UGVC_AFR_NEW_CONTIG: CHROM differs from the previous line's, or the first record
+ * of the call) and *out_n_filtered (records that get new_filter).  UGVC_E_DATA where the reference raises: ugvc_afr_error gives the record (index in this call) and the
+ * UGVC_AFR_E_* reason (-1 / 0 for a data error of the index pass, see ugvc_last_data_error). */
+int ugvc_afr_bgzf(ugvc_ctx* ctx, int lane, const uint8_t* data, size_t n_bytes, uint32_t skip_head, uint64_t take_bytes,
+                  int is_text, const ugvc_afr_params* params, uint8_t* out_bgzf, size_t out_capacity, size_t* out_bytes,
+                  uint32_t* out_block_csize, size_t block_capacity, size_t* out_n_blocks, ugvc_recinfo* out_recinfo,
+                  int64_t* out_line_start, int64_t* out_end, uint8_t* out_flags, size_t capacity_records,
+                  int64_t* out_n_records, int64_t* out_n_filtered);
+int ugvc_afr_error(const ugvc_ctx* ctx, int lane, int64_t* out_record, int32_t* out_reason);
+/* ms of the last ugvc_afr_bgzf call on `lane` between CUDA events: H2D + inflate, index K1, decide + scan + copy,
+ * deflate + pack, D2H. */
+int ugvc_afr_stage_ms(ugvc_ctx* ctx, int lane, float out_ms[5]);
+/* Test hook: decide, scan and copy on the caller's records (line_start: n + 1 entries, every line ending with '\n'),
+ * without a context.  Returns the bytes written to out, UGVC_E_DATA with *out_err_record / *out_err_reason where the
+ * reference raises (nothing written). */
+int64_t ugvc_test_afr(const uint8_t* text, size_t n_bytes, const int64_t* line_start, int64_t n, const ugvc_afr_params* params,
+                      uint8_t* out, size_t capacity, int64_t* out_line_start, uint8_t* out_failed, int64_t* out_end,
+                      int64_t* out_n_filtered, int64_t* out_err_record, int32_t* out_err_reason);
+
 /* ---- test hook ------------------------------------------------------------ */
 /* K1's numeric-literal parser (csrc/numparse.h) compiled for the host: parses one token of
  * `text` (NUL-terminated); returns 0 ok / 1 missing (".") / 2 not exactly parseable. */

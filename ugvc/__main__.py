@@ -14,6 +14,7 @@ if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
 TOOLS = {"filter_variants_pipeline": "variantcalling_b200.filter_variants_pipeline",
+         "filter_low_af_ratio_to_background": "variantcalling_b200.low_af_ratio",
          "evaluate_concordance": "variantcalling_b200.evaluate_concordance"}
 
 

@@ -13,6 +13,7 @@
 #include "deflate.cuh"
 #ifndef UGVC_HOST_EMU
 #include "fileio.cuh"
+#include "low_af_ratio.cuh"
 #include "multiallelic.cuh"
 #endif
 
@@ -69,6 +70,14 @@ struct Lane {
         float ms[5] = {0, 0, 0, 0, 0};
         cudaEvent_t ev_split[9] = {};  // ugvc_filter_bgzf_split: created at its first call on the lane
         float ms_split[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+        // ugvc_afr_bgzf: scan aggregates (grown on demand), totals {bytes, failed} + error word, pinned copies
+        int64_t* d_afr_agg = nullptr;
+        size_t cap_afr_agg = 0;
+        int64_t* d_afr_tot = nullptr;         // [2] totals, then the error word
+        int64_t* h_afr_tot = nullptr;         // pinned, same layout
+        float ms_afr[5] = {0, 0, 0, 0, 0};
+        int64_t afr_err_record = -1;
+        int32_t afr_err_reason = 0;
     } fb;
 };
 
@@ -189,6 +198,9 @@ static void free_lane(Lane& l) {
     cudaFree(l.fb.d_bl_pos);
     cudaFree(l.fb.d_bl_meta);
     if (l.fb.h_total) cudaFreeHost(l.fb.h_total);
+    cudaFree(l.fb.d_afr_agg);
+    cudaFree(l.fb.d_afr_tot);
+    if (l.fb.h_afr_tot) cudaFreeHost(l.fb.h_afr_tot);
     for (auto& e : l.fb.ev)
         if (e) cudaEventDestroy(e);
     for (auto& e : l.fb.ev_split)
@@ -1364,6 +1376,12 @@ extern "C" int ugvc_test_device_deflate(ugvc_ctx* ctx, const uint8_t*, size_t, i
                                         size_t*) {
     return fail(ctx, UGVC_E_STATE, "the device BGZF encoder is not part of the host emulation");
 }
+extern "C" int ugvc_afr_bgzf(ugvc_ctx* ctx, int, const uint8_t*, size_t, uint32_t, uint64_t, int, const ugvc_afr_params*, uint8_t*,
+                             size_t, size_t*, uint32_t*, size_t, size_t*, ugvc_recinfo*, int64_t*, int64_t*, uint8_t*, size_t, int64_t*, int64_t*) {
+    return fail(ctx, UGVC_E_STATE, "the device file path of filter_low_af_ratio_to_background is not part of the host emulation");
+}
+extern "C" int ugvc_afr_error(const ugvc_ctx*, int, int64_t*, int32_t*) { return UGVC_E_STATE; }
+extern "C" int ugvc_afr_stage_ms(ugvc_ctx*, int, float*) { return UGVC_E_STATE; }
 #else
 #define FIO_BL_NAMES_AT (8 * (UGVC_MAX_BLACKLISTS + 1) + 4 * (UGVC_MAX_BLACKLISTS + 2))
 #define FIO_BL_META (FIO_BL_NAMES_AT + UGVC_MAX_BLACKLIST_NAME_BYTES)
@@ -1944,6 +1962,147 @@ extern "C" int ugvc_test_device_deflate(ugvc_ctx* ctx, const uint8_t* data, size
     if (n_blocks) memcpy(out_block_csize, f.h_bsize.data(), (size_t)n_blocks * sizeof(uint32_t));
     *out_bytes = packed;
     *out_n_blocks = (size_t)n_blocks;
+    return UGVC_OK;
+}
+
+// filter_low_af_ratio_to_background, file to file: inflate (or upload) -> index K1 -> afr decide / scan / copy -> deflate
+extern "C" int ugvc_afr_bgzf(ugvc_ctx* ctx, int lane, const uint8_t* data, size_t n_bytes, uint32_t skip_head, uint64_t take_bytes,
+                             int is_text, const ugvc_afr_params* params, uint8_t* out_bgzf, size_t out_capacity, size_t* out_bytes,
+                             uint32_t* out_block_csize, size_t block_capacity, size_t* out_n_blocks, ugvc_recinfo* out_recinfo,
+                             int64_t* out_line_start, int64_t* out_end, uint8_t* out_flags, size_t capacity_records,
+                             int64_t* out_n_records, int64_t* out_n_filtered) {
+    if (!ctx) return UGVC_E_ARG;
+    AfrDev P;
+    if (!afr_params(params, &P)) return fail(ctx, UGVC_E_ARG, "afr_bgzf: bad params");
+    if (!ctx->has_plan || ctx->lanes.empty()) return fail(ctx, UGVC_E_STATE, "afr_bgzf: load the model-less plan and reserve first");
+    if (lane < 0 || lane >= (int)ctx->lanes.size()) return fail(ctx, UGVC_E_ARG, "afr_bgzf: lane out of range");
+    if (!data || !n_bytes || !out_bgzf || !out_bytes || !out_n_records || !out_n_filtered || (is_text && skip_head))
+        return fail(ctx, UGVC_E_ARG, "afr_bgzf: bad argument");
+    CU(cudaSetDevice(ctx->device));
+    Lane& l = ctx->lanes[lane];
+    if (l.submitted) return fail(ctx, UGVC_E_STATE, "afr_bgzf: lane already has a batch in flight");
+    int rc = file_bufs(ctx, l);
+    if (rc) return rc;
+    Lane::FileBufs& f = l.fb;
+    f.afr_err_record = -1;
+    f.afr_err_reason = 0;
+    cudaStream_t st = l.stream;
+    (void)cudaGetLastError();
+    if (!f.d_afr_tot) {
+        CU(cudaMalloc(&f.d_afr_tot, 3 * sizeof(int64_t)));
+        CU(cudaHostAlloc(&f.h_afr_tot, 3 * sizeof(int64_t), cudaHostAllocDefault));
+    }
+    const size_t need_agg = 2 * (l.b.cap_records / AFR_CHUNK + 2);
+    if (need_agg > f.cap_afr_agg) {
+        cudaFree(f.d_afr_agg);
+        f.d_afr_agg = nullptr;
+        f.cap_afr_agg = 0;
+        CU(cudaMalloc(&f.d_afr_agg, need_agg * sizeof(int64_t)));
+        f.cap_afr_agg = need_agg;
+    }
+    CU(cudaEventRecord(f.ev[0], st));
+    // ---- the range's text on the device, its first byte 16-byte aligned
+    const uint8_t* d_text = nullptr;
+    size_t n_text = 0;
+    if (is_text) {
+        if (n_bytes > ctx->cap_bytes) return fail(ctx, UGVC_E_ARG, "afr_bgzf: text larger than the reserved max_bytes");
+        n_text = take_bytes ? (size_t)take_bytes : n_bytes;
+        if (n_text > n_bytes) return fail(ctx, UGVC_E_ARG, "afr_bgzf: take_bytes beyond the text");
+        CU(cudaMemcpyAsync(l.d_text, data, n_text, cudaMemcpyHostToDevice, st));
+        CU(cudaMemsetAsync(l.d_text + n_text, '\n', TEXT_SLACK, st));
+        d_text = l.d_text;
+    } else {
+        const size_t shift = (16 - (skip_head & 15u)) & 15u;
+        size_t total = 0;
+        rc = stage_bgzf(ctx, l, data, n_bytes, inflate_decoder(), &total, shift);
+        if (rc) return rc;
+        if (skip_head > total) return fail(ctx, UGVC_E_ARG, "afr_bgzf: skip_head beyond the inflated blocks");
+        n_text = take_bytes ? (size_t)take_bytes : total - skip_head;
+        if (skip_head + n_text > total) return fail(ctx, UGVC_E_ARG, "afr_bgzf: the range is longer than the inflated blocks");
+        d_text = l.d_text + shift + skip_head;
+    }
+    CU(cudaEventRecord(f.ev[1], st));
+    // ---- index pass: line starts, POS, len(REF)
+    rc = enqueue_kernels(ctx, l, d_text, n_text, 0.0, l.b.low_score, l.b.probs, l.b.qual, l.b.recinfo, l.b.line_start,
+                         l.b.cap_records, l.b.n_records, st);
+    if (rc) return rc;
+    CU(cudaMemcpyAsync(l.h_n, l.b.n_records, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(l.h_err, l.d_err, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+    CU(cudaEventRecord(f.ev[2], st));
+    CU(cudaStreamSynchronize(st));
+    if (!is_text && l.h_inf_err && *l.h_inf_err) {
+        const int code = *l.h_inf_err;
+        *l.h_inf_err = 0;
+        return fail(ctx, UGVC_E_IO, inf_err_message(code));
+    }
+    rc = decode_error(ctx, *l.h_err);
+    if (rc) return rc;
+    const int64_t n = *l.h_n;
+    l.last_n = n;
+    *out_n_records = n;
+    if ((size_t)n > capacity_records) return fail(ctx, UGVC_E_ARG, "afr_bgzf: output capacity smaller than the record count");
+    // ---- decide, scan, copy
+    CU(cudaMemsetAsync(f.d_afr_tot, 0xFF, 3 * sizeof(int64_t), st));
+    afr_launch_decide(d_text, l.b.line_start, n, P, f.d_score, f.d_len, f.d_end, f.d_out_ls, f.d_afr_agg, f.d_afr_tot,
+                      reinterpret_cast<unsigned long long*>(f.d_afr_tot + 2), ctx->sm_count, st);
+    CU(cudaGetLastError());
+    if (n == 0) CU(cudaMemsetAsync(f.d_afr_tot, 0, 2 * sizeof(int64_t), st));
+    CU(cudaMemcpyAsync(f.h_afr_tot, f.d_afr_tot, 3 * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    const unsigned long long err = (unsigned long long)f.h_afr_tot[2];
+    if (err != AFR_NO_ERROR) {
+        f.afr_err_record = (int64_t)(err >> 4);
+        f.afr_err_reason = (int32_t)(err & 0xF);
+        return fail(ctx, UGVC_E_DATA, "afr_bgzf: the reference raises at record " + std::to_string(f.afr_err_record) + " (reason " +
+                                          std::to_string(f.afr_err_reason) + ")");
+    }
+    const size_t out_text = (size_t)f.h_afr_tot[0];
+    const int64_t n_failed = f.h_afr_tot[1];
+    if (out_text > f.cap_out) return fail(ctx, UGVC_E_ARG, "afr_bgzf: the written text exceeds the writer's buffer");
+    if (n == 0) CU(cudaMemsetAsync(f.d_out_ls, 0, sizeof(int64_t), st));
+    afr_launch_copy(d_text, l.b.line_start, n, P, f.d_score, f.d_out_ls, f.d_out_text, ctx->sm_count, st);
+    CU(cudaMemsetAsync(f.d_out_text + out_text, 0, 16, st));  // the encoder reads whole words
+    CU(cudaEventRecord(f.ev[3], st));
+    // ---- deflate, pack
+    const int n_blocks = (int)((out_text + DEF_CHUNK - 1) / DEF_CHUNK);
+    if ((size_t)n_blocks > f.cap_blocks || (out_block_csize && (size_t)n_blocks > block_capacity))
+        return fail(ctx, UGVC_E_ARG, "afr_bgzf: more output blocks than room for them");
+    rc = encode_blocks(ctx, f, out_text, n_blocks, deflate_encoder(), st);
+    if (rc) return rc;
+    f.h_bsize.resize((size_t)n_blocks + 1);
+    if (n_blocks) CU(cudaMemcpyAsync(f.h_bsize.data(), f.d_bsize, (size_t)n_blocks * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+    CU(cudaEventRecord(f.ev[4], st));
+    CU(cudaStreamSynchronize(st));
+    size_t packed = 0;
+    for (int b = 0; b < n_blocks; ++b) packed += f.h_bsize[b];
+    if (packed > out_capacity) return fail(ctx, UGVC_E_ARG, "afr_bgzf: out_capacity smaller than the compressed output");
+    ctx->launches += 9;
+    // ---- results to the host
+    if (packed) CU(cudaMemcpyAsync(out_bgzf, f.d_packed, packed, cudaMemcpyDeviceToHost, st));
+    if (out_block_csize && n_blocks) memcpy(out_block_csize, f.h_bsize.data(), (size_t)n_blocks * sizeof(uint32_t));
+    if (out_recinfo && n) CU(cudaMemcpyAsync(out_recinfo, l.b.recinfo, (size_t)n * sizeof(ugvc_recinfo), cudaMemcpyDeviceToHost, st));
+    if (out_line_start) CU(cudaMemcpyAsync(out_line_start, f.d_out_ls, (size_t)(n + 1) * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    if (out_end && n) CU(cudaMemcpyAsync(out_end, f.d_end, (size_t)n * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    if (out_flags && n) CU(cudaMemcpyAsync(out_flags, f.d_score, (size_t)n, cudaMemcpyDeviceToHost, st));
+    CU(cudaEventRecord(f.ev[5], st));
+    CU(cudaStreamSynchronize(st));
+    *out_bytes = packed;
+    *out_n_filtered = n_failed;
+    if (out_n_blocks) *out_n_blocks = (size_t)n_blocks;
+    for (int k = 0; k < 5; ++k) cudaEventElapsedTime(&f.ms_afr[k], f.ev[k], f.ev[k + 1]);
+    return UGVC_OK;
+}
+
+extern "C" int ugvc_afr_error(const ugvc_ctx* ctx, int lane, int64_t* out_record, int32_t* out_reason) {
+    if (!ctx || lane < 0 || lane >= (int)ctx->lanes.size() || !out_record || !out_reason) return UGVC_E_ARG;
+    *out_record = ctx->lanes[lane].fb.afr_err_record;
+    *out_reason = ctx->lanes[lane].fb.afr_err_reason;
+    return UGVC_OK;
+}
+
+extern "C" int ugvc_afr_stage_ms(ugvc_ctx* ctx, int lane, float out_ms[5]) {
+    if (!ctx || lane < 0 || lane >= (int)ctx->lanes.size() || !out_ms) return UGVC_E_ARG;
+    memcpy(out_ms, ctx->lanes[lane].fb.ms_afr, sizeof(ctx->lanes[lane].fb.ms_afr));
     return UGVC_OK;
 }
 #endif  // !UGVC_HOST_EMU

@@ -42,6 +42,19 @@ class FileEdits(C.Structure):
                 ("blacklist_name_off", C.c_void_p), ("out_end", C.c_void_p), ("n_blacklisted", C.c_int64)]
 
 
+class AfrParams(C.Structure):
+    """ugvc_afr_params (include/ugvc_b200.h)."""
+    _fields_ = [("af_ratio_threshold", C.c_double), ("af_ratio_threshold_h_indels", C.c_double), ("t_vaf_threshold", C.c_double),
+                ("new_filter", C.c_char_p), ("new_filter_len", C.c_int32), ("variant_type_kind", C.c_int32),
+                ("vaf_kind", C.c_int32), ("vaf_integer", C.c_int32), ("bg_vaf_kind", C.c_int32), ("bg_vaf_integer", C.c_int32)]
+
+
+AFR_KIND_NONE, AFR_KIND_SCALAR, AFR_KIND_TUPLE = 0, 1, 2
+AFR_E_LITERAL, AFR_E_TYPE = 1, 2
+AFR_FAILED, AFR_REWRITTEN, AFR_NEW_CONTIG = 1, 2, 4
+AFR_MAX_FILTER_BYTES = 63
+
+
 class Counts(C.Structure):
     _fields_ = [("n_records", C.c_int64), ("n_low_score", C.c_int64), ("n_pass", C.c_int64), ("n_cg", C.c_int64)]
 
@@ -146,14 +159,23 @@ SIGNATURES = {
     "ugvc_filter_bgzf_first_records": (C.c_int, [_vp, C.c_int, _vp, C.c_int, _vp]),
     "ugvc_test_parse_float": (C.c_int, [C.c_char_p, C.POINTER(C.c_float), C.POINTER(C.c_double),
                                         C.POINTER(C.c_int)]),
+    "ugvc_afr_bgzf": (C.c_int, [_vp, C.c_int, _vp, _sz, C.c_uint32, C.c_uint64, C.c_int, C.POINTER(AfrParams), _vp, _sz,
+                                C.POINTER(_sz), _vp, _sz, C.POINTER(_sz), _vp, _vp, _vp, _vp, _sz, _i64p, _i64p]),
+    "ugvc_afr_error": (C.c_int, [_vp, C.c_int, _i64p, C.POINTER(C.c_int32)]),
+    "ugvc_afr_stage_ms": (C.c_int, [_vp, C.c_int, _vp]),
+    "ugvc_test_afr": (C.c_int64, [_vp, _sz, _vp, C.c_int64, C.POINTER(AfrParams), _vp, _sz, _vp, _vp, _vp, _i64p, _i64p,
+                                  C.POINTER(C.c_int32)]),
 }
 
 # the concordance-frame annotation entry points are bound on first use (load_annotation), so that a build of the
 # library without them, such as the host emulation of the filter path, still loads
 _BOUND_ON_USE = frozenset(n for n in SIGNATURES if n.startswith("ugvc_conc_annot"))
+# so are those of filter_low_af_ratio_to_background (load_low_af_ratio)
+_AFR_BOUND_ON_USE = frozenset(n for n in SIGNATURES if n.startswith(("ugvc_afr_", "ugvc_test_afr")))
 
 _lib = None
 _annotation_bound = False
+_afr_bound = False
 
 
 def load_library() -> C.CDLL:
@@ -166,7 +188,7 @@ def load_library() -> C.CDLL:
                 f"(make -C variantcalling_b200/csrc).  There is no CPU fallback for the hot path.")
         lib = C.CDLL(LIB_PATH)
         for name, (res, args) in SIGNATURES.items():
-            if name in _BOUND_ON_USE:
+            if name in _BOUND_ON_USE or name in _AFR_BOUND_ON_USE:
                 continue
             fn = getattr(lib, name)
             fn.restype = res
@@ -186,6 +208,20 @@ def load_annotation() -> C.CDLL:
             fn.restype = res
             fn.argtypes = args
         _annotation_bound = True
+    return lib
+
+
+def load_low_af_ratio() -> C.CDLL:
+    """load_library() with the filter_low_af_ratio_to_background entry points bound.  Raises if the library lacks them."""
+    global _afr_bound  # noqa: PLW0603
+    lib = load_library()
+    if not _afr_bound:
+        for name in sorted(_AFR_BOUND_ON_USE):
+            res, args = SIGNATURES[name]
+            fn = getattr(lib, name)
+            fn.restype = res
+            fn.argtypes = args
+        _afr_bound = True
     return lib
 
 
@@ -500,6 +536,41 @@ class Context:
         return {"n_records": k, "bgzf": out[: nb.value], "block_csize": blocks[: nblk.value], "recinfo": ri[:k],
                 "line_start": ls[: k + 1], "low_score": low[:k]}
 
+    def afr_bgzf(self, data: np.ndarray, skip_head: int, take_bytes: int, is_text: bool, params: AfrParams, max_records: int,
+                 lane: int = 0) -> dict:
+        """filter_low_af_ratio_to_background on one range of whole lines (ugvc_afr_bgzf): BGZF blocks (or, with is_text,
+        the plain text) in, BGZF blocks of the edited records out.  Needs the model-less plan and reserve() sized for the
+        range.  A record the reference raises at comes back as UgvcDataError with .afr_record / .afr_reason set."""
+        lib = load_low_af_ratio()
+        src = np.ascontiguousarray(data, dtype=np.uint8)
+        n_text = take_bytes or (src.size if is_text else src.size * 64)
+        out = np.empty(n_text // DEF_CHUNK * 65536 + n_text // 8 + max_records * (AFR_MAX_FILTER_BYTES + 1) + (1 << 20), np.uint8)
+        blocks = np.empty(out.size // 65536 + 8, dtype=np.uint32)
+        ri = np.empty(max(1, max_records), dtype=RECINFO_DTYPE)
+        ls = np.empty(max_records + 1, dtype=np.int64)
+        end = np.empty(max(1, max_records), dtype=np.int64)
+        flags = np.empty(max(1, max_records), dtype=np.uint8)
+        nb, nblk, n, nf = C.c_size_t(), C.c_size_t(), C.c_int64(), C.c_int64()
+        rc = lib.ugvc_afr_bgzf(self.h, lane, _ptr(src), src.size, skip_head, take_bytes, int(bool(is_text)), C.byref(params),
+                               _ptr(out), out.size, C.byref(nb), _ptr(blocks), blocks.size, C.byref(nblk), _ptr(ri), _ptr(ls),
+                               _ptr(end), _ptr(flags), max_records, C.byref(n), C.byref(nf))
+        if rc == UGVC_E_DATA:
+            rec, reason = C.c_int64(), C.c_int32()
+            lib.ugvc_afr_error(self.h, lane, C.byref(rec), C.byref(reason))
+            err = UgvcDataError(rc, lib.ugvc_last_error(self.h).decode())
+            err.afr_record, err.afr_reason = int(rec.value), int(reason.value)
+            raise err
+        self._check(rc)
+        k = n.value
+        return {"n_records": k, "n_filtered": int(nf.value), "bgzf": out[: nb.value], "block_csize": blocks[: nblk.value],
+                "recinfo": ri[:k], "line_start": ls[: k + 1], "end": end[:k], "flags": flags[:k]}
+
+    def afr_stage_ms(self, lane: int = 0) -> list[float]:
+        """ms of the last afr_bgzf call on `lane`: H2D + inflate, index K1, decide + scan + copy, deflate + pack, D2H."""
+        ms = (C.c_float * 5)()
+        self._check(load_low_af_ratio().ugvc_afr_stage_ms(self.h, lane, C.cast(ms, C.c_void_p)))
+        return list(ms)
+
     def filter_bgzf_first_records(self, text_offsets, lane: int = 0) -> np.ndarray:
         """Index of the first record at or after each byte offset of the last filter_bgzf range's text."""
         off = np.ascontiguousarray(text_offsets, dtype=np.uint64)
@@ -630,6 +701,29 @@ class Context:
         n = C.c_int64()
         self._check(self.lib.ugvc_stage_ms(self.h, arr, C.byref(n)))
         return list(arr), n.value
+
+
+def test_afr(text: bytes, params: AfrParams) -> dict:
+    """The filter_low_af_ratio_to_background kernels alone on whole lines (test hook ugvc_test_afr, no context):
+    {"text", "line_start", "failed", "end", "n_filtered"}, or {"error": (record, reason)} where the reference raises."""
+    lib = load_low_af_ratio()
+    buf = np.frombuffer(text, dtype=np.uint8)
+    nl = np.flatnonzero(buf == 10)  # noqa: PLR2004
+    ls = np.concatenate(([0], nl + 1)).astype(np.int64)
+    n = ls.size - 1
+    out = np.empty(buf.size + n * (AFR_MAX_FILTER_BYTES + 1) + 16, np.uint8)
+    out_ls = np.empty(n + 1, np.int64)
+    failed = np.empty(max(1, n), np.uint8)
+    end = np.empty(max(1, n), np.int64)
+    nf, rec, reason = C.c_int64(), C.c_int64(), C.c_int32()
+    nb = lib.ugvc_test_afr(_ptr(buf) if buf.size else None, buf.size, _ptr(ls), n, C.byref(params), _ptr(out), out.size,
+                           _ptr(out_ls), _ptr(failed), _ptr(end), C.byref(nf), C.byref(rec), C.byref(reason))
+    if nb == UGVC_E_DATA:
+        return {"error": (int(rec.value), int(reason.value))}
+    if nb < 0:
+        raise UgvcError(int(nb), "ugvc_test_afr failed")
+    return {"text": out[:nb].tobytes(), "line_start": out_ls, "failed": failed[:n].astype(bool), "end": end[:n],
+            "n_filtered": int(nf.value)}
 
 
 def synth_header(n_custom: int) -> str:
