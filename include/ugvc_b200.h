@@ -531,6 +531,67 @@ int64_t ugvc_test_afr(const uint8_t* text, size_t n_bytes, const int64_t* line_s
                       uint8_t* out, size_t capacity, int64_t* out_line_start, uint8_t* out_failed, int64_t* out_end,
                       int64_t* out_n_filtered, int64_t* out_err_record, int32_t* out_err_reason);
 
+/* ---- calibrate_bridging_snvs on the device (DESIGN.md 4d) ------------------
+ * Replaces the per-record loop of ugvc/pipelines/vcfbed/calibrate_bridging_snvs.py (run, :91-130; is_homopolymer_snp,
+ * :9-66): a non-PASS single-base SNV with QUAL >= min_initial_qual whose ALT base extends a reference homopolymer to at
+ * least min_query_hmer_size (not a tandem repeat, both sides at least min_distance_from_edge long) and whose sample 0
+ * has sum(AD[1:]) / DP >= min_tumor_vaf, sum(BG_AD[1:]) / max(0.01, BG_DP) <= max_normal_vaf and
+ * BG_DP > min_normal_depth is rescued: QUAL becomes qual_text and FILTER "PASS".  Every other byte is kept as read.
+ * The FASTA window is read from the context's contig table (ugvc_bsn_add_contig), bytes compared as stored.
+ *   *_kind  UGVC_BSN_KIND_*: how the header declares AD / DP / BG_AD / BG_DP; *_integer: Type=Integer (else Float) */
+#define UGVC_BSN_KIND_NONE 0    /* not declared: reading it raises KeyError */
+#define UGVC_BSN_KIND_SCALAR 1  /* Number=1 */
+#define UGVC_BSN_KIND_TUPLE 2   /* any other Number */
+#define UGVC_BSN_MAX_QUAL_BYTES 31
+#define UGVC_BSN_E_LITERAL 1        /* a QUAL / AD / DP / BG_AD / BG_DP literal the parser refuses (numparse.h) */
+#define UGVC_BSN_E_TYPE 2           /* TypeError: None or a tuple where a number is needed, a slice of a scalar, ALT "." */
+#define UGVC_BSN_E_ZERO_DIVISION 3  /* ZeroDivisionError: DP is 0 */
+#define UGVC_BSN_E_KEY 4            /* KeyError: a rescue key missing from the header or the record's FORMAT / sample */
+#define UGVC_BSN_E_FETCH 5          /* ValueError of FastaFile.fetch: negative window start or contig not in the FASTA */
+#define UGVC_BSN_RESCUED 1
+#define UGVC_BSN_NEW_CONTIG 4
+typedef struct ugvc_bsn_params {
+    int32_t min_query_hmer_size;     /* >= 0 */
+    int32_t min_distance_from_edge;
+    double min_initial_qual;
+    double min_tumor_vaf;
+    double max_normal_vaf;
+    double min_normal_depth;
+    const char* qual_text;           /* the rescued QUAL column, 1..UGVC_BSN_MAX_QUAL_BYTES bytes, not NUL-terminated */
+    int32_t qual_len;
+    int32_t ad_kind, ad_integer;
+    int32_t dp_kind, dp_integer;
+    int32_t bg_ad_kind, bg_ad_integer;
+    int32_t bg_dp_kind, bg_dp_integer;
+} ugvc_bsn_params;
+/* Contigs of the FASTA stay on the context until ugvc_bsn_clear_contigs or ugvc_free: one copy of the raw bytes (case
+ * kept) per name; adding a name again replaces its bytes. */
+int ugvc_bsn_add_contig(ugvc_ctx* ctx, const char* name, const uint8_t* seq, int64_t len);
+int ugvc_bsn_clear_contigs(ugvc_ctx* ctx);
+/* One range of whole VCF data lines per call, in the shape and with the outputs of ugvc_afr_bgzf; out_flags holds
+ * UGVC_BSN_RESCUED | UGVC_BSN_NEW_CONTIG, out_hmer (may be NULL) the hmer_size of each record whose window was walked
+ * (0 elsewhere), out_src_line_start (may be NULL; n + 1 entries) the line starts in the range's input text, and
+ * *out_n_rescued the rescued count.  UGVC_E_DATA where the reference raises: ugvc_bsn_error gives the record (index in
+ * this call) and the UGVC_BSN_E_* reason (-1 / 0 for a data error of the index pass, see ugvc_last_data_error). */
+int ugvc_bsn_bgzf(ugvc_ctx* ctx, int lane, const uint8_t* data, size_t n_bytes, uint32_t skip_head, uint64_t take_bytes,
+                  int is_text, const ugvc_bsn_params* params, uint8_t* out_bgzf, size_t out_capacity, size_t* out_bytes,
+                  uint32_t* out_block_csize, size_t block_capacity, size_t* out_n_blocks, ugvc_recinfo* out_recinfo,
+                  int64_t* out_line_start, int64_t* out_src_line_start, int64_t* out_end, uint8_t* out_flags,
+                  int32_t* out_hmer, size_t capacity_records, int64_t* out_n_records, int64_t* out_n_rescued);
+int ugvc_bsn_error(const ugvc_ctx* ctx, int lane, int64_t* out_record, int32_t* out_reason);
+/* ms of the last ugvc_bsn_bgzf call on `lane` between CUDA events: H2D + inflate, index K1, decide + scan + copy,
+ * deflate + pack, D2H. */
+int ugvc_bsn_stage_ms(ugvc_ctx* ctx, int lane, float out_ms[5]);
+/* Test hook: decide, scan and copy on the caller's records (line_start: n + 1 entries, every line ending with '\n')
+ * and contigs (n_contigs names at names[name_off[k] .. name_off[k+1]), bytes at seq[seq_off[k] .. seq_off[k+1])), without
+ * a context.  Returns the bytes written to out, UGVC_E_DATA with *out_err_record / *out_err_reason where the reference
+ * raises (nothing written). */
+int64_t ugvc_test_bsn(const uint8_t* text, size_t n_bytes, const int64_t* line_start, int64_t n, const uint8_t* names,
+                      const int64_t* name_off, const uint8_t* seq, const int64_t* seq_off, int32_t n_contigs,
+                      const ugvc_bsn_params* params, uint8_t* out, size_t capacity, int64_t* out_line_start,
+                      uint8_t* out_rescued, int32_t* out_hmer, int64_t* out_end, int64_t* out_n_rescued,
+                      int64_t* out_err_record, int32_t* out_err_reason);
+
 /* ---- test hook ------------------------------------------------------------ */
 /* K1's numeric-literal parser (csrc/numparse.h) compiled for the host: parses one token of
  * `text` (NUL-terminated); returns 0 ok / 1 missing (".") / 2 not exactly parseable. */

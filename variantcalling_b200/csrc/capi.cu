@@ -14,6 +14,7 @@
 #ifndef UGVC_HOST_EMU
 #include "fileio.cuh"
 #include "low_af_ratio.cuh"
+#include "bridging_snvs.cuh"
 #include "multiallelic.cuh"
 #endif
 
@@ -78,6 +79,12 @@ struct Lane {
         float ms_afr[5] = {0, 0, 0, 0, 0};
         int64_t afr_err_record = -1;
         int32_t afr_err_reason = 0;
+        // ugvc_bsn_bgzf (shares the scan scratch and totals above): hmer_size of each record, grown on demand
+        int32_t* d_bsn_hmer = nullptr;
+        size_t cap_bsn_hmer = 0;
+        float ms_bsn[5] = {0, 0, 0, 0, 0};
+        int64_t bsn_err_record = -1;
+        int32_t bsn_err_reason = 0;
     } fb;
 };
 
@@ -117,6 +124,15 @@ struct ugvc_ctx {
     float stage_ms[4] = {0, 0, 0, 0};
     int64_t err_record = -1;
     int32_t err_column = -1, err_reason = 0;
+#ifndef UGVC_HOST_EMU
+    // calibrate_bridging_snvs: the FASTA contigs (device copies) and their sorted table, rebuilt when a contig changes
+    std::vector<std::string> bsn_names;
+    std::vector<uint8_t*> bsn_seq;
+    std::vector<int64_t> bsn_len;
+    BsnTable bsn_table;
+    bool bsn_dirty = false;
+    std::mutex bsn_mu;
+#endif
 };
 
 static std::string g_init_error;
@@ -201,6 +217,7 @@ static void free_lane(Lane& l) {
     cudaFree(l.fb.d_afr_agg);
     cudaFree(l.fb.d_afr_tot);
     if (l.fb.h_afr_tot) cudaFreeHost(l.fb.h_afr_tot);
+    cudaFree(l.fb.d_bsn_hmer);
     for (auto& e : l.fb.ev)
         if (e) cudaEventDestroy(e);
     for (auto& e : l.fb.ev_split)
@@ -236,6 +253,10 @@ extern "C" void ugvc_free(ugvc_ctx* ctx) {
     cudaFree(ctx->d_slot_kind);
     cudaFree(ctx->d_def_tables);
     cudaFree(ctx->d_counts);
+#ifndef UGVC_HOST_EMU
+    for (uint8_t* p : ctx->bsn_seq) cudaFree(p);
+    bsn_table_free(&ctx->bsn_table);
+#endif
     delete ctx;
 }
 
@@ -1382,6 +1403,17 @@ extern "C" int ugvc_afr_bgzf(ugvc_ctx* ctx, int, const uint8_t*, size_t, uint32_
 }
 extern "C" int ugvc_afr_error(const ugvc_ctx*, int, int64_t*, int32_t*) { return UGVC_E_STATE; }
 extern "C" int ugvc_afr_stage_ms(ugvc_ctx*, int, float*) { return UGVC_E_STATE; }
+extern "C" int ugvc_bsn_add_contig(ugvc_ctx* ctx, const char*, const uint8_t*, int64_t) {
+    return fail(ctx, UGVC_E_STATE, "the device file path of calibrate_bridging_snvs is not part of the host emulation");
+}
+extern "C" int ugvc_bsn_clear_contigs(ugvc_ctx*) { return UGVC_E_STATE; }
+extern "C" int ugvc_bsn_bgzf(ugvc_ctx* ctx, int, const uint8_t*, size_t, uint32_t, uint64_t, int, const ugvc_bsn_params*, uint8_t*,
+                             size_t, size_t*, uint32_t*, size_t, size_t*, ugvc_recinfo*, int64_t*, int64_t*, int64_t*, uint8_t*,
+                             int32_t*, size_t, int64_t*, int64_t*) {
+    return fail(ctx, UGVC_E_STATE, "the device file path of calibrate_bridging_snvs is not part of the host emulation");
+}
+extern "C" int ugvc_bsn_error(const ugvc_ctx*, int, int64_t*, int32_t*) { return UGVC_E_STATE; }
+extern "C" int ugvc_bsn_stage_ms(ugvc_ctx*, int, float*) { return UGVC_E_STATE; }
 #else
 #define FIO_BL_NAMES_AT (8 * (UGVC_MAX_BLACKLISTS + 1) + 4 * (UGVC_MAX_BLACKLISTS + 2))
 #define FIO_BL_META (FIO_BL_NAMES_AT + UGVC_MAX_BLACKLIST_NAME_BYTES)
@@ -1965,27 +1997,14 @@ extern "C" int ugvc_test_device_deflate(ugvc_ctx* ctx, const uint8_t* data, size
     return UGVC_OK;
 }
 
-// filter_low_af_ratio_to_background, file to file: inflate (or upload) -> index K1 -> afr decide / scan / copy -> deflate
-extern "C" int ugvc_afr_bgzf(ugvc_ctx* ctx, int lane, const uint8_t* data, size_t n_bytes, uint32_t skip_head, uint64_t take_bytes,
-                             int is_text, const ugvc_afr_params* params, uint8_t* out_bgzf, size_t out_capacity, size_t* out_bytes,
-                             uint32_t* out_block_csize, size_t block_capacity, size_t* out_n_blocks, ugvc_recinfo* out_recinfo,
-                             int64_t* out_line_start, int64_t* out_end, uint8_t* out_flags, size_t capacity_records,
-                             int64_t* out_n_records, int64_t* out_n_filtered) {
-    if (!ctx) return UGVC_E_ARG;
-    AfrDev P;
-    if (!afr_params(params, &P)) return fail(ctx, UGVC_E_ARG, "afr_bgzf: bad params");
-    if (!ctx->has_plan || ctx->lanes.empty()) return fail(ctx, UGVC_E_STATE, "afr_bgzf: load the model-less plan and reserve first");
-    if (lane < 0 || lane >= (int)ctx->lanes.size()) return fail(ctx, UGVC_E_ARG, "afr_bgzf: lane out of range");
-    if (!data || !n_bytes || !out_bgzf || !out_bytes || !out_n_records || !out_n_filtered || (is_text && skip_head))
-        return fail(ctx, UGVC_E_ARG, "afr_bgzf: bad argument");
-    CU(cudaSetDevice(ctx->device));
-    Lane& l = ctx->lanes[lane];
-    if (l.submitted) return fail(ctx, UGVC_E_STATE, "afr_bgzf: lane already has a batch in flight");
+// The first half of a VCF-to-VCF tool call (ugvc_afr_bgzf, ugvc_bsn_bgzf): the scan scratch, the range's text on the
+// device (inflated, or uploaded plain) and the index pass (line starts, POS, len(REF)); events ev[0..2].
+static int tool_front(ugvc_ctx* ctx, Lane& l, const char* who, const uint8_t* data, size_t n_bytes, uint32_t skip_head,
+                      uint64_t take_bytes, int is_text, size_t capacity_records, const uint8_t** d_text_out, int64_t* n_out) {
+    const std::string w(who);
     int rc = file_bufs(ctx, l);
     if (rc) return rc;
     Lane::FileBufs& f = l.fb;
-    f.afr_err_record = -1;
-    f.afr_err_reason = 0;
     cudaStream_t st = l.stream;
     (void)cudaGetLastError();
     if (!f.d_afr_tot) {
@@ -2005,9 +2024,9 @@ extern "C" int ugvc_afr_bgzf(ugvc_ctx* ctx, int lane, const uint8_t* data, size_
     const uint8_t* d_text = nullptr;
     size_t n_text = 0;
     if (is_text) {
-        if (n_bytes > ctx->cap_bytes) return fail(ctx, UGVC_E_ARG, "afr_bgzf: text larger than the reserved max_bytes");
+        if (n_bytes > ctx->cap_bytes) return fail(ctx, UGVC_E_ARG, w + ": text larger than the reserved max_bytes");
         n_text = take_bytes ? (size_t)take_bytes : n_bytes;
-        if (n_text > n_bytes) return fail(ctx, UGVC_E_ARG, "afr_bgzf: take_bytes beyond the text");
+        if (n_text > n_bytes) return fail(ctx, UGVC_E_ARG, w + ": take_bytes beyond the text");
         CU(cudaMemcpyAsync(l.d_text, data, n_text, cudaMemcpyHostToDevice, st));
         CU(cudaMemsetAsync(l.d_text + n_text, '\n', TEXT_SLACK, st));
         d_text = l.d_text;
@@ -2016,9 +2035,9 @@ extern "C" int ugvc_afr_bgzf(ugvc_ctx* ctx, int lane, const uint8_t* data, size_
         size_t total = 0;
         rc = stage_bgzf(ctx, l, data, n_bytes, inflate_decoder(), &total, shift);
         if (rc) return rc;
-        if (skip_head > total) return fail(ctx, UGVC_E_ARG, "afr_bgzf: skip_head beyond the inflated blocks");
+        if (skip_head > total) return fail(ctx, UGVC_E_ARG, w + ": skip_head beyond the inflated blocks");
         n_text = take_bytes ? (size_t)take_bytes : total - skip_head;
-        if (skip_head + n_text > total) return fail(ctx, UGVC_E_ARG, "afr_bgzf: the range is longer than the inflated blocks");
+        if (skip_head + n_text > total) return fail(ctx, UGVC_E_ARG, w + ": the range is longer than the inflated blocks");
         d_text = l.d_text + shift + skip_head;
     }
     CU(cudaEventRecord(f.ev[1], st));
@@ -2039,8 +2058,72 @@ extern "C" int ugvc_afr_bgzf(ugvc_ctx* ctx, int lane, const uint8_t* data, size_
     if (rc) return rc;
     const int64_t n = *l.h_n;
     l.last_n = n;
-    *out_n_records = n;
-    if ((size_t)n > capacity_records) return fail(ctx, UGVC_E_ARG, "afr_bgzf: output capacity smaller than the record count");
+    *n_out = n;
+    if ((size_t)n > capacity_records) return fail(ctx, UGVC_E_ARG, w + ": output capacity smaller than the record count");
+    *d_text_out = d_text;
+    return UGVC_OK;
+}
+
+// The second half, after the tool's copy kernel has written out_text bytes at fb.d_out_text: deflate and pack (events
+// ev[3..4]), then the D2H of the blocks, recinfo and the output line starts is enqueued; the caller adds its own copies,
+// records ev[5] and synchronizes.
+static int tool_back(ugvc_ctx* ctx, Lane& l, const char* who, size_t out_text, int64_t n, uint8_t* out_bgzf, size_t out_capacity,
+                     size_t* out_bytes, uint32_t* out_block_csize, size_t block_capacity, size_t* out_n_blocks,
+                     ugvc_recinfo* out_recinfo, int64_t* out_line_start) {
+    const std::string w(who);
+    Lane::FileBufs& f = l.fb;
+    cudaStream_t st = l.stream;
+    CU(cudaMemsetAsync(f.d_out_text + out_text, 0, 16, st));  // the encoder reads whole words
+    CU(cudaEventRecord(f.ev[3], st));
+    // ---- deflate, pack
+    const int n_blocks = (int)((out_text + DEF_CHUNK - 1) / DEF_CHUNK);
+    if ((size_t)n_blocks > f.cap_blocks || (out_block_csize && (size_t)n_blocks > block_capacity))
+        return fail(ctx, UGVC_E_ARG, w + ": more output blocks than room for them");
+    int rc = encode_blocks(ctx, f, out_text, n_blocks, deflate_encoder(), st);
+    if (rc) return rc;
+    f.h_bsize.resize((size_t)n_blocks + 1);
+    if (n_blocks) CU(cudaMemcpyAsync(f.h_bsize.data(), f.d_bsize, (size_t)n_blocks * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+    CU(cudaEventRecord(f.ev[4], st));
+    CU(cudaStreamSynchronize(st));
+    size_t packed = 0;
+    for (int b = 0; b < n_blocks; ++b) packed += f.h_bsize[b];
+    if (packed > out_capacity) return fail(ctx, UGVC_E_ARG, w + ": out_capacity smaller than the compressed output");
+    ctx->launches += 9;
+    // ---- results to the host
+    if (packed) CU(cudaMemcpyAsync(out_bgzf, f.d_packed, packed, cudaMemcpyDeviceToHost, st));
+    if (out_block_csize && n_blocks) memcpy(out_block_csize, f.h_bsize.data(), (size_t)n_blocks * sizeof(uint32_t));
+    if (out_recinfo && n) CU(cudaMemcpyAsync(out_recinfo, l.b.recinfo, (size_t)n * sizeof(ugvc_recinfo), cudaMemcpyDeviceToHost, st));
+    if (out_line_start) CU(cudaMemcpyAsync(out_line_start, f.d_out_ls, (size_t)(n + 1) * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    *out_bytes = packed;
+    if (out_n_blocks) *out_n_blocks = (size_t)n_blocks;
+    return UGVC_OK;
+}
+
+// filter_low_af_ratio_to_background, file to file: inflate (or upload) -> index K1 -> afr decide / scan / copy -> deflate
+extern "C" int ugvc_afr_bgzf(ugvc_ctx* ctx, int lane, const uint8_t* data, size_t n_bytes, uint32_t skip_head, uint64_t take_bytes,
+                             int is_text, const ugvc_afr_params* params, uint8_t* out_bgzf, size_t out_capacity, size_t* out_bytes,
+                             uint32_t* out_block_csize, size_t block_capacity, size_t* out_n_blocks, ugvc_recinfo* out_recinfo,
+                             int64_t* out_line_start, int64_t* out_end, uint8_t* out_flags, size_t capacity_records,
+                             int64_t* out_n_records, int64_t* out_n_filtered) {
+    if (!ctx) return UGVC_E_ARG;
+    AfrDev P;
+    if (!afr_params(params, &P)) return fail(ctx, UGVC_E_ARG, "afr_bgzf: bad params");
+    if (!ctx->has_plan || ctx->lanes.empty()) return fail(ctx, UGVC_E_STATE, "afr_bgzf: load the model-less plan and reserve first");
+    if (lane < 0 || lane >= (int)ctx->lanes.size()) return fail(ctx, UGVC_E_ARG, "afr_bgzf: lane out of range");
+    if (!data || !n_bytes || !out_bgzf || !out_bytes || !out_n_records || !out_n_filtered || (is_text && skip_head))
+        return fail(ctx, UGVC_E_ARG, "afr_bgzf: bad argument");
+    CU(cudaSetDevice(ctx->device));
+    Lane& l = ctx->lanes[lane];
+    if (l.submitted) return fail(ctx, UGVC_E_STATE, "afr_bgzf: lane already has a batch in flight");
+    Lane::FileBufs& f = l.fb;
+    f.afr_err_record = -1;
+    f.afr_err_reason = 0;
+    const uint8_t* d_text = nullptr;
+    int64_t n = 0;
+    int rc = tool_front(ctx, l, "afr_bgzf", data, n_bytes, skip_head, take_bytes, is_text, capacity_records, &d_text, &n);
+    *out_n_records = n;  // set before a failed capacity check too
+    if (rc) return rc;
+    cudaStream_t st = l.stream;
     // ---- decide, scan, copy
     CU(cudaMemsetAsync(f.d_afr_tot, 0xFF, 3 * sizeof(int64_t), st));
     afr_launch_decide(d_text, l.b.line_start, n, P, f.d_score, f.d_len, f.d_end, f.d_out_ls, f.d_afr_agg, f.d_afr_tot,
@@ -2061,34 +2144,14 @@ extern "C" int ugvc_afr_bgzf(ugvc_ctx* ctx, int lane, const uint8_t* data, size_
     if (out_text > f.cap_out) return fail(ctx, UGVC_E_ARG, "afr_bgzf: the written text exceeds the writer's buffer");
     if (n == 0) CU(cudaMemsetAsync(f.d_out_ls, 0, sizeof(int64_t), st));
     afr_launch_copy(d_text, l.b.line_start, n, P, f.d_score, f.d_out_ls, f.d_out_text, ctx->sm_count, st);
-    CU(cudaMemsetAsync(f.d_out_text + out_text, 0, 16, st));  // the encoder reads whole words
-    CU(cudaEventRecord(f.ev[3], st));
-    // ---- deflate, pack
-    const int n_blocks = (int)((out_text + DEF_CHUNK - 1) / DEF_CHUNK);
-    if ((size_t)n_blocks > f.cap_blocks || (out_block_csize && (size_t)n_blocks > block_capacity))
-        return fail(ctx, UGVC_E_ARG, "afr_bgzf: more output blocks than room for them");
-    rc = encode_blocks(ctx, f, out_text, n_blocks, deflate_encoder(), st);
+    rc = tool_back(ctx, l, "afr_bgzf", out_text, n, out_bgzf, out_capacity, out_bytes, out_block_csize, block_capacity, out_n_blocks,
+                   out_recinfo, out_line_start);
     if (rc) return rc;
-    f.h_bsize.resize((size_t)n_blocks + 1);
-    if (n_blocks) CU(cudaMemcpyAsync(f.h_bsize.data(), f.d_bsize, (size_t)n_blocks * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-    CU(cudaEventRecord(f.ev[4], st));
-    CU(cudaStreamSynchronize(st));
-    size_t packed = 0;
-    for (int b = 0; b < n_blocks; ++b) packed += f.h_bsize[b];
-    if (packed > out_capacity) return fail(ctx, UGVC_E_ARG, "afr_bgzf: out_capacity smaller than the compressed output");
-    ctx->launches += 9;
-    // ---- results to the host
-    if (packed) CU(cudaMemcpyAsync(out_bgzf, f.d_packed, packed, cudaMemcpyDeviceToHost, st));
-    if (out_block_csize && n_blocks) memcpy(out_block_csize, f.h_bsize.data(), (size_t)n_blocks * sizeof(uint32_t));
-    if (out_recinfo && n) CU(cudaMemcpyAsync(out_recinfo, l.b.recinfo, (size_t)n * sizeof(ugvc_recinfo), cudaMemcpyDeviceToHost, st));
-    if (out_line_start) CU(cudaMemcpyAsync(out_line_start, f.d_out_ls, (size_t)(n + 1) * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
     if (out_end && n) CU(cudaMemcpyAsync(out_end, f.d_end, (size_t)n * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
     if (out_flags && n) CU(cudaMemcpyAsync(out_flags, f.d_score, (size_t)n, cudaMemcpyDeviceToHost, st));
     CU(cudaEventRecord(f.ev[5], st));
     CU(cudaStreamSynchronize(st));
-    *out_bytes = packed;
     *out_n_filtered = n_failed;
-    if (out_n_blocks) *out_n_blocks = (size_t)n_blocks;
     for (int k = 0; k < 5; ++k) cudaEventElapsedTime(&f.ms_afr[k], f.ev[k], f.ev[k + 1]);
     return UGVC_OK;
 }
@@ -2103,6 +2166,140 @@ extern "C" int ugvc_afr_error(const ugvc_ctx* ctx, int lane, int64_t* out_record
 extern "C" int ugvc_afr_stage_ms(ugvc_ctx* ctx, int lane, float out_ms[5]) {
     if (!ctx || lane < 0 || lane >= (int)ctx->lanes.size() || !out_ms) return UGVC_E_ARG;
     memcpy(out_ms, ctx->lanes[lane].fb.ms_afr, sizeof(ctx->lanes[lane].fb.ms_afr));
+    return UGVC_OK;
+}
+
+// ---- calibrate_bridging_snvs: the contig table, then file to file as ugvc_afr_bgzf with the bsn kernels
+extern "C" int ugvc_bsn_add_contig(ugvc_ctx* ctx, const char* name, const uint8_t* seq, int64_t len) {
+    if (!ctx) return UGVC_E_ARG;
+    if (!name || len < 0 || (len > 0 && !seq)) return fail(ctx, UGVC_E_ARG, "bsn_add_contig: bad arguments");
+    CU(cudaSetDevice(ctx->device));
+    std::lock_guard<std::mutex> g(ctx->bsn_mu);
+    uint8_t* d = nullptr;
+    CU(cudaMalloc(&d, (size_t)(len ? len : 1)));
+    if (len) {
+        const cudaError_t e = cudaMemcpy(d, seq, (size_t)len, cudaMemcpyHostToDevice);
+        if (e != cudaSuccess) {
+            cudaFree(d);
+            return fail(ctx, UGVC_E_CUDA, std::string("bsn_add_contig: ") + cudaGetErrorString(e));
+        }
+    }
+    size_t k = 0;
+    while (k < ctx->bsn_names.size() && ctx->bsn_names[k] != name) ++k;
+    if (k < ctx->bsn_names.size()) {
+        CU(cudaDeviceSynchronize());  // no call may still read the old bytes
+        cudaFree(ctx->bsn_seq[k]);
+        ctx->bsn_seq[k] = d;
+        ctx->bsn_len[k] = len;
+    } else {
+        ctx->bsn_names.emplace_back(name);
+        ctx->bsn_seq.push_back(d);
+        ctx->bsn_len.push_back(len);
+    }
+    ctx->bsn_dirty = true;
+    return UGVC_OK;
+}
+
+extern "C" int ugvc_bsn_clear_contigs(ugvc_ctx* ctx) {
+    if (!ctx) return UGVC_E_ARG;
+    CU(cudaSetDevice(ctx->device));
+    std::lock_guard<std::mutex> g(ctx->bsn_mu);
+    CU(cudaDeviceSynchronize());
+    for (uint8_t* p : ctx->bsn_seq) cudaFree(p);
+    ctx->bsn_names.clear();
+    ctx->bsn_seq.clear();
+    ctx->bsn_len.clear();
+    bsn_table_free(&ctx->bsn_table);
+    ctx->bsn_dirty = false;
+    return UGVC_OK;
+}
+
+extern "C" int ugvc_bsn_bgzf(ugvc_ctx* ctx, int lane, const uint8_t* data, size_t n_bytes, uint32_t skip_head, uint64_t take_bytes,
+                             int is_text, const ugvc_bsn_params* params, uint8_t* out_bgzf, size_t out_capacity, size_t* out_bytes,
+                             uint32_t* out_block_csize, size_t block_capacity, size_t* out_n_blocks, ugvc_recinfo* out_recinfo,
+                             int64_t* out_line_start, int64_t* out_src_line_start, int64_t* out_end, uint8_t* out_flags,
+                             int32_t* out_hmer, size_t capacity_records, int64_t* out_n_records, int64_t* out_n_rescued) {
+    if (!ctx) return UGVC_E_ARG;
+    BsnDev P;
+    if (!bsn_params(params, &P)) return fail(ctx, UGVC_E_ARG, "bsn_bgzf: bad params");
+    if (!ctx->has_plan || ctx->lanes.empty()) return fail(ctx, UGVC_E_STATE, "bsn_bgzf: load the model-less plan and reserve first");
+    if (lane < 0 || lane >= (int)ctx->lanes.size()) return fail(ctx, UGVC_E_ARG, "bsn_bgzf: lane out of range");
+    if (!data || !n_bytes || !out_bgzf || !out_bytes || !out_n_records || !out_n_rescued || (is_text && skip_head))
+        return fail(ctx, UGVC_E_ARG, "bsn_bgzf: bad argument");
+    CU(cudaSetDevice(ctx->device));
+    Lane& l = ctx->lanes[lane];
+    if (l.submitted) return fail(ctx, UGVC_E_STATE, "bsn_bgzf: lane already has a batch in flight");
+    BsnContigs C;
+    {
+        std::lock_guard<std::mutex> g(ctx->bsn_mu);
+        if (ctx->bsn_dirty) {
+            CU(cudaDeviceSynchronize());  // no call may still read the old table
+            std::vector<const uint8_t*> seq(ctx->bsn_seq.begin(), ctx->bsn_seq.end());
+            CU(bsn_table_build(ctx->bsn_names, seq, ctx->bsn_len, &ctx->bsn_table));
+            ctx->bsn_dirty = false;
+        }
+        C = ctx->bsn_table.view();
+    }
+    Lane::FileBufs& f = l.fb;
+    f.bsn_err_record = -1;
+    f.bsn_err_reason = 0;
+    const uint8_t* d_text = nullptr;
+    int64_t n = 0;
+    int rc = tool_front(ctx, l, "bsn_bgzf", data, n_bytes, skip_head, take_bytes, is_text, capacity_records, &d_text, &n);
+    *out_n_records = n;
+    if (rc) return rc;
+    cudaStream_t st = l.stream;
+    if (l.b.cap_records > f.cap_bsn_hmer) {
+        cudaFree(f.d_bsn_hmer);
+        f.d_bsn_hmer = nullptr;
+        f.cap_bsn_hmer = 0;
+        CU(cudaMalloc(&f.d_bsn_hmer, (l.b.cap_records ? l.b.cap_records : 1) * sizeof(int32_t)));
+        f.cap_bsn_hmer = l.b.cap_records;
+    }
+    // ---- decide, scan, copy
+    CU(cudaMemsetAsync(f.d_afr_tot, 0xFF, 3 * sizeof(int64_t), st));
+    bsn_launch_decide(d_text, l.b.line_start, n, P, C, f.d_score, f.d_bsn_hmer, f.d_len, f.d_end, f.d_out_ls, f.d_afr_agg,
+                      f.d_afr_tot, reinterpret_cast<unsigned long long*>(f.d_afr_tot + 2), ctx->sm_count, st);
+    CU(cudaGetLastError());
+    if (n == 0) CU(cudaMemsetAsync(f.d_afr_tot, 0, 2 * sizeof(int64_t), st));
+    CU(cudaMemcpyAsync(f.h_afr_tot, f.d_afr_tot, 3 * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    const unsigned long long err = (unsigned long long)f.h_afr_tot[2];
+    if (err != AFR_NO_ERROR) {
+        f.bsn_err_record = (int64_t)(err >> 4);
+        f.bsn_err_reason = (int32_t)(err & 0xF);
+        return fail(ctx, UGVC_E_DATA, "bsn_bgzf: the reference raises at record " + std::to_string(f.bsn_err_record) + " (reason " +
+                                          std::to_string(f.bsn_err_reason) + ")");
+    }
+    const size_t out_text = (size_t)f.h_afr_tot[0];
+    const int64_t n_rescued = f.h_afr_tot[1];
+    if (out_text > f.cap_out) return fail(ctx, UGVC_E_ARG, "bsn_bgzf: the written text exceeds the writer's buffer");
+    if (n == 0) CU(cudaMemsetAsync(f.d_out_ls, 0, sizeof(int64_t), st));
+    bsn_launch_copy(d_text, l.b.line_start, n, P, f.d_score, f.d_out_ls, f.d_out_text, ctx->sm_count, st);
+    rc = tool_back(ctx, l, "bsn_bgzf", out_text, n, out_bgzf, out_capacity, out_bytes, out_block_csize, block_capacity, out_n_blocks,
+                   out_recinfo, out_line_start);
+    if (rc) return rc;
+    if (out_src_line_start) CU(cudaMemcpyAsync(out_src_line_start, l.b.line_start, (size_t)(n + 1) * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    if (out_end && n) CU(cudaMemcpyAsync(out_end, f.d_end, (size_t)n * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    if (out_flags && n) CU(cudaMemcpyAsync(out_flags, f.d_score, (size_t)n, cudaMemcpyDeviceToHost, st));
+    if (out_hmer && n) CU(cudaMemcpyAsync(out_hmer, f.d_bsn_hmer, (size_t)n * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    CU(cudaEventRecord(f.ev[5], st));
+    CU(cudaStreamSynchronize(st));
+    *out_n_rescued = n_rescued;
+    for (int k = 0; k < 5; ++k) cudaEventElapsedTime(&f.ms_bsn[k], f.ev[k], f.ev[k + 1]);
+    return UGVC_OK;
+}
+
+extern "C" int ugvc_bsn_error(const ugvc_ctx* ctx, int lane, int64_t* out_record, int32_t* out_reason) {
+    if (!ctx || lane < 0 || lane >= (int)ctx->lanes.size() || !out_record || !out_reason) return UGVC_E_ARG;
+    *out_record = ctx->lanes[lane].fb.bsn_err_record;
+    *out_reason = ctx->lanes[lane].fb.bsn_err_reason;
+    return UGVC_OK;
+}
+
+extern "C" int ugvc_bsn_stage_ms(ugvc_ctx* ctx, int lane, float out_ms[5]) {
+    if (!ctx || lane < 0 || lane >= (int)ctx->lanes.size() || !out_ms) return UGVC_E_ARG;
+    memcpy(out_ms, ctx->lanes[lane].fb.ms_bsn, sizeof(ctx->lanes[lane].fb.ms_bsn));
     return UGVC_OK;
 }
 #endif  // !UGVC_HOST_EMU

@@ -23,6 +23,10 @@ bool afr_params(const ugvc_afr_params* p, AfrDev* d);
 void afr_launch_decide(const uint8_t* text, const int64_t* line_start, int64_t n, const AfrDev& P, uint8_t* flags,
                        int64_t* len, int64_t* end, int64_t* out_ls, int64_t* agg, int64_t* totals,
                        unsigned long long* err, int sm_count, cudaStream_t st);
+// The scan step of afr_launch_decide alone, also used by the calibrate_bridging_snvs kernels (bridging_snvs.cu): the
+// exclusive scan of len (n entries) into out_ls, totals[0] = the summed bytes, totals[1] = records with flags bit 0 set.
+void afr_launch_scan(const int64_t* len, const uint8_t* flags, int64_t n, int64_t* out_ls, int64_t* agg, int64_t* totals,
+                     int sm_count, cudaStream_t st);
 // every line with its new FILTER column, at out + out_ls[i]
 void afr_launch_copy(const uint8_t* text, const int64_t* line_start, int64_t n, const AfrDev& P, const uint8_t* flags,
                      const int64_t* out_ls, uint8_t* out, int sm_count, cudaStream_t st);

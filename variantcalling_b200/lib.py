@@ -55,6 +55,21 @@ AFR_FAILED, AFR_REWRITTEN, AFR_NEW_CONTIG = 1, 2, 4
 AFR_MAX_FILTER_BYTES = 63
 
 
+class BsnParams(C.Structure):
+    """ugvc_bsn_params (include/ugvc_b200.h)."""
+    _fields_ = [("min_query_hmer_size", C.c_int32), ("min_distance_from_edge", C.c_int32), ("min_initial_qual", C.c_double),
+                ("min_tumor_vaf", C.c_double), ("max_normal_vaf", C.c_double), ("min_normal_depth", C.c_double),
+                ("qual_text", C.c_char_p), ("qual_len", C.c_int32), ("ad_kind", C.c_int32), ("ad_integer", C.c_int32),
+                ("dp_kind", C.c_int32), ("dp_integer", C.c_int32), ("bg_ad_kind", C.c_int32), ("bg_ad_integer", C.c_int32),
+                ("bg_dp_kind", C.c_int32), ("bg_dp_integer", C.c_int32)]
+
+
+BSN_KIND_NONE, BSN_KIND_SCALAR, BSN_KIND_TUPLE = 0, 1, 2
+BSN_E_LITERAL, BSN_E_TYPE, BSN_E_ZERO_DIVISION, BSN_E_KEY, BSN_E_FETCH = 1, 2, 3, 4, 5
+BSN_RESCUED, BSN_NEW_CONTIG = 1, 4
+BSN_MAX_QUAL_BYTES = 31
+
+
 class Counts(C.Structure):
     _fields_ = [("n_records", C.c_int64), ("n_low_score", C.c_int64), ("n_pass", C.c_int64), ("n_cg", C.c_int64)]
 
@@ -165,6 +180,14 @@ SIGNATURES = {
     "ugvc_afr_stage_ms": (C.c_int, [_vp, C.c_int, _vp]),
     "ugvc_test_afr": (C.c_int64, [_vp, _sz, _vp, C.c_int64, C.POINTER(AfrParams), _vp, _sz, _vp, _vp, _vp, _i64p, _i64p,
                                   C.POINTER(C.c_int32)]),
+    "ugvc_bsn_add_contig": (C.c_int, [_vp, C.c_char_p, _vp, C.c_int64]),
+    "ugvc_bsn_clear_contigs": (C.c_int, [_vp]),
+    "ugvc_bsn_bgzf": (C.c_int, [_vp, C.c_int, _vp, _sz, C.c_uint32, C.c_uint64, C.c_int, C.POINTER(BsnParams), _vp, _sz,
+                                C.POINTER(_sz), _vp, _sz, C.POINTER(_sz), _vp, _vp, _vp, _vp, _vp, _vp, _sz, _i64p, _i64p]),
+    "ugvc_bsn_error": (C.c_int, [_vp, C.c_int, _i64p, C.POINTER(C.c_int32)]),
+    "ugvc_bsn_stage_ms": (C.c_int, [_vp, C.c_int, _vp]),
+    "ugvc_test_bsn": (C.c_int64, [_vp, _sz, _vp, C.c_int64, _vp, _vp, _vp, _vp, C.c_int32, C.POINTER(BsnParams), _vp, _sz,
+                                  _vp, _vp, _vp, _vp, _i64p, _i64p, C.POINTER(C.c_int32)]),
 }
 
 # the concordance-frame annotation entry points are bound on first use (load_annotation), so that a build of the
@@ -172,10 +195,13 @@ SIGNATURES = {
 _BOUND_ON_USE = frozenset(n for n in SIGNATURES if n.startswith("ugvc_conc_annot"))
 # so are those of filter_low_af_ratio_to_background (load_low_af_ratio)
 _AFR_BOUND_ON_USE = frozenset(n for n in SIGNATURES if n.startswith(("ugvc_afr_", "ugvc_test_afr")))
+# and those of calibrate_bridging_snvs (load_bridging_snvs)
+_BSN_BOUND_ON_USE = frozenset(n for n in SIGNATURES if n.startswith(("ugvc_bsn_", "ugvc_test_bsn")))
 
 _lib = None
 _annotation_bound = False
 _afr_bound = False
+_bsn_bound = False
 
 
 def load_library() -> C.CDLL:
@@ -188,7 +214,7 @@ def load_library() -> C.CDLL:
                 f"(make -C variantcalling_b200/csrc).  There is no CPU fallback for the hot path.")
         lib = C.CDLL(LIB_PATH)
         for name, (res, args) in SIGNATURES.items():
-            if name in _BOUND_ON_USE or name in _AFR_BOUND_ON_USE:
+            if name in _BOUND_ON_USE or name in _AFR_BOUND_ON_USE or name in _BSN_BOUND_ON_USE:
                 continue
             fn = getattr(lib, name)
             fn.restype = res
@@ -222,6 +248,20 @@ def load_low_af_ratio() -> C.CDLL:
             fn.restype = res
             fn.argtypes = args
         _afr_bound = True
+    return lib
+
+
+def load_bridging_snvs() -> C.CDLL:
+    """load_library() with the calibrate_bridging_snvs entry points bound.  Raises if the library lacks them."""
+    global _bsn_bound  # noqa: PLW0603
+    lib = load_library()
+    if not _bsn_bound:
+        for name in sorted(_BSN_BOUND_ON_USE):
+            res, args = SIGNATURES[name]
+            fn = getattr(lib, name)
+            fn.restype = res
+            fn.argtypes = args
+        _bsn_bound = True
     return lib
 
 
@@ -571,6 +611,52 @@ class Context:
         self._check(load_low_af_ratio().ugvc_afr_stage_ms(self.h, lane, C.cast(ms, C.c_void_p)))
         return list(ms)
 
+    def bsn_add_contig(self, name: str, seq: bytes):
+        """Upload one FASTA contig (raw bytes) to the context's calibrate_bridging_snvs contig table."""
+        buf = np.frombuffer(seq, dtype=np.uint8)
+        self._check(load_bridging_snvs().ugvc_bsn_add_contig(self.h, name.encode(), _ptr(buf) if buf.size else None, buf.size))
+
+    def bsn_clear_contigs(self):
+        self._check(load_bridging_snvs().ugvc_bsn_clear_contigs(self.h))
+
+    def bsn_bgzf(self, data: np.ndarray, skip_head: int, take_bytes: int, is_text: bool, params: BsnParams, max_records: int,
+                 lane: int = 0) -> dict:
+        """calibrate_bridging_snvs on one range of whole lines (ugvc_bsn_bgzf), in the shape of afr_bgzf, plus "hmer" and
+        "src_line_start" (line starts in the range's input text).  A record the reference raises at comes back as
+        UgvcDataError with .bsn_record / .bsn_reason set."""
+        lib = load_bridging_snvs()
+        src = np.ascontiguousarray(data, dtype=np.uint8)
+        n_text = take_bytes or (src.size if is_text else src.size * 64)
+        out = np.empty(n_text // DEF_CHUNK * 65536 + n_text // 8 + max_records * (BSN_MAX_QUAL_BYTES + 5) + (1 << 20), np.uint8)
+        blocks = np.empty(out.size // 65536 + 8, dtype=np.uint32)
+        ri = np.empty(max(1, max_records), dtype=RECINFO_DTYPE)
+        ls = np.empty(max_records + 1, dtype=np.int64)
+        src_ls = np.empty(max_records + 1, dtype=np.int64)
+        end = np.empty(max(1, max_records), dtype=np.int64)
+        flags = np.empty(max(1, max_records), dtype=np.uint8)
+        hmer = np.empty(max(1, max_records), dtype=np.int32)
+        nb, nblk, n, nr = C.c_size_t(), C.c_size_t(), C.c_int64(), C.c_int64()
+        rc = lib.ugvc_bsn_bgzf(self.h, lane, _ptr(src), src.size, skip_head, take_bytes, int(bool(is_text)), C.byref(params),
+                               _ptr(out), out.size, C.byref(nb), _ptr(blocks), blocks.size, C.byref(nblk), _ptr(ri), _ptr(ls),
+                               _ptr(src_ls), _ptr(end), _ptr(flags), _ptr(hmer), max_records, C.byref(n), C.byref(nr))
+        if rc == UGVC_E_DATA:
+            rec, reason = C.c_int64(), C.c_int32()
+            lib.ugvc_bsn_error(self.h, lane, C.byref(rec), C.byref(reason))
+            err = UgvcDataError(rc, lib.ugvc_last_error(self.h).decode())
+            err.bsn_record, err.bsn_reason = int(rec.value), int(reason.value)
+            raise err
+        self._check(rc)
+        k = n.value
+        return {"n_records": k, "n_rescued": int(nr.value), "bgzf": out[: nb.value], "block_csize": blocks[: nblk.value],
+                "recinfo": ri[:k], "line_start": ls[: k + 1], "src_line_start": src_ls[: k + 1], "end": end[:k],
+                "flags": flags[:k], "hmer": hmer[:k]}
+
+    def bsn_stage_ms(self, lane: int = 0) -> list[float]:
+        """ms of the last bsn_bgzf call on `lane`: H2D + inflate, index K1, decide + scan + copy, deflate + pack, D2H."""
+        ms = (C.c_float * 5)()
+        self._check(load_bridging_snvs().ugvc_bsn_stage_ms(self.h, lane, C.cast(ms, C.c_void_p)))
+        return list(ms)
+
     def filter_bgzf_first_records(self, text_offsets, lane: int = 0) -> np.ndarray:
         """Index of the first record at or after each byte offset of the last filter_bgzf range's text."""
         off = np.ascontiguousarray(text_offsets, dtype=np.uint64)
@@ -724,6 +810,37 @@ def test_afr(text: bytes, params: AfrParams) -> dict:
         raise UgvcError(int(nb), "ugvc_test_afr failed")
     return {"text": out[:nb].tobytes(), "line_start": out_ls, "failed": failed[:n].astype(bool), "end": end[:n],
             "n_filtered": int(nf.value)}
+
+
+def test_bsn(text: bytes, contigs: dict, params: BsnParams) -> dict:
+    """The calibrate_bridging_snvs kernels alone on whole lines and the given contigs ({name: bytes}; test hook
+    ugvc_test_bsn, no context): {"text", "line_start", "rescued", "hmer", "end", "n_rescued"}, or {"error": (record,
+    reason)} where the reference raises."""
+    lib = load_bridging_snvs()
+    buf = np.frombuffer(text, dtype=np.uint8)
+    nl = np.flatnonzero(buf == 10)  # noqa: PLR2004
+    ls = np.concatenate(([0], nl + 1)).astype(np.int64)
+    n = ls.size - 1
+    names = [k.encode() for k in contigs]
+    name_buf = np.frombuffer(b"".join(names) or b"\0", dtype=np.uint8)
+    name_off = np.concatenate(([0], np.cumsum([len(k) for k in names]))).astype(np.int64)
+    seq_buf = np.frombuffer(b"".join(contigs.values()) or b"\0", dtype=np.uint8)
+    seq_off = np.concatenate(([0], np.cumsum([len(v) for v in contigs.values()]))).astype(np.int64)
+    out = np.empty(buf.size + n * (BSN_MAX_QUAL_BYTES + 5) + 16, np.uint8)
+    out_ls = np.empty(n + 1, np.int64)
+    rescued = np.empty(max(1, n), np.uint8)
+    hmer = np.empty(max(1, n), np.int32)
+    end = np.empty(max(1, n), np.int64)
+    nr, rec, reason = C.c_int64(), C.c_int64(), C.c_int32()
+    nb = lib.ugvc_test_bsn(_ptr(buf) if buf.size else None, buf.size, _ptr(ls), n, _ptr(name_buf), _ptr(name_off), _ptr(seq_buf),
+                           _ptr(seq_off), len(names), C.byref(params), _ptr(out), out.size, _ptr(out_ls), _ptr(rescued),
+                           _ptr(hmer), _ptr(end), C.byref(nr), C.byref(rec), C.byref(reason))
+    if nb == UGVC_E_DATA:
+        return {"error": (int(rec.value), int(reason.value))}
+    if nb < 0:
+        raise UgvcError(int(nb), "ugvc_test_bsn failed")
+    return {"text": out[:nb].tobytes(), "line_start": out_ls, "rescued": rescued[:n].astype(bool), "hmer": hmer[:n],
+            "end": end[:n], "n_rescued": int(nr.value)}
 
 
 def synth_header(n_custom: int) -> str:
