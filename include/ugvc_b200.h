@@ -364,15 +364,20 @@ int ugvc_filter_bgzf_first_records(ugvc_ctx* ctx, int lane, const uint64_t* text
  * the final FILTER is PASS), cls (0 fp, 1 tp, 2 fn, 3 tn: the classify / classify_gt column), indel,
  * hmer_len (hmer_indel_length, < 0 for null), group (NULL = derive from indel / hmer_len, else the
  * caller's group id per record, -1 = none).  Inputs are host arrays, or device arrays when
- * inputs_on_device != 0.
- *   out_counts[g][6]   = tp, fp, missed (call < truth), initial_tp, n_called (not fn), n_fn
+ * inputs_on_device != 0.  A group id outside -1..6 or a cls code above 3 anywhere in the input makes the
+ * call return UGVC_E_ARG with every output zero.
+ *   out_counts[g][8]   = tp, fp, missed (call < truth), initial_tp, n_called (not fn), n_fn,
+ *                        n_nan, n_inf (called records whose score is NaN / +-inf: where sklearn's
+ *                        assert_all_finite raises, the Python mirror raises; the curve is still drawn)
  *   out_curve_len[g]   = points of the raw precision/recall curve kept on the device (0 for g = 8)
  *   out_cutoff[g]      = the 20th largest score of the group (stats_utils.py:202-207)
  *   out_selected[g][2] = number of called records, number of true ones among them
  * ugvc_conc_curve copies group g's raw curve: precision = tps/(tps+fps), recall = tps/tps[-1] at each
- * distinct score, in increasing-threshold order (sklearn's order, without its final (1, 0) point). */
+ * distinct score, in increasing-threshold order (sklearn's order, without its final (1, 0) point).  The
+ * threshold of a run of equal scores is its first score in input order, so a run of -0.0 and +0.0 reports
+ * the sign of its first zero (scikit-learn 1.5, the reference's pin). */
 #define UGVC_CONC_GROUPS 9
-#define UGVC_CONC_COUNTERS 6
+#define UGVC_CONC_COUNTERS 8
 typedef struct ugvc_conc ugvc_conc;
 int ugvc_conc_create(int device, ugvc_conc** out);
 void ugvc_conc_free(ugvc_conc* h);

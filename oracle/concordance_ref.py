@@ -40,7 +40,20 @@ def default_group(indel: np.ndarray, hmer: np.ndarray) -> np.ndarray:
     return out
 
 
+def assert_all_finite(y_score: np.ndarray):
+    """sklearn.utils.assert_all_finite as _binary_clf_curve calls it: NaN's message before inf's."""
+    if y_score.dtype.kind != "f":
+        return
+    if np.isnan(y_score).any():
+        raise ValueError("Input contains NaN.")
+    if np.isinf(y_score).any():
+        raise ValueError(f"Input contains infinity or a value too large for {y_score.dtype!r}.")
+
+
 def sklearn_pr_curve(y_true: np.ndarray, y_score: np.ndarray):
+    """A run of equal scores reports its first score in input order (the stable ascending sort, reversed, keeps
+    the run's last index, which is its first in input order): a run of -0.0 and +0.0 keeps its first zero's sign."""
+    assert_all_finite(y_score)
     order = np.argsort(y_score, kind="mergesort")[::-1]
     y_score, y_true = y_score[order], y_true[order]
     idx = np.r_[np.where(np.diff(y_score))[0], y_true.size - 1]

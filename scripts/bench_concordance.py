@@ -55,7 +55,7 @@ def main():
     # device-resident inputs
     d = [torch.from_numpy(a).cuda() for a in (scores, pred, cls, indel.astype(np.uint8), hmer)]
     L = lib.load_library()
-    counts = np.zeros((9, 6), np.int64)
+    counts = np.zeros((PC.N_GROUPS, PC.N_COUNTERS), np.int64)
     clen, cut, sel = np.zeros(9, np.int64), np.zeros(9), np.zeros((9, 2), np.int64)
     p = lib._ptr  # noqa: SLF001
 

@@ -16,6 +16,7 @@ extern "C" int ugvc_conc_create(int, ugvc_conc**) { return UGVC_E_CUDA; }
 extern "C" void ugvc_conc_free(ugvc_conc*) {}
 extern "C" const char* ugvc_conc_last_error(const ugvc_conc*) { return NOT_EMULATED; }
 extern "C" long long ugvc_conc_launch_count(const ugvc_conc*) { return 0; }
+// ugvc_conc_run writes UGVC_CONC_GROUPS x UGVC_CONC_COUNTERS (9 x 8) counters on the device; refused here
 extern "C" int ugvc_conc_run(ugvc_conc*, int64_t, const double*, const uint8_t*, const uint8_t*, const uint8_t*, const int32_t*,
                              const int8_t*, int, int, int64_t*, int64_t*, double*, int64_t*) { return UGVC_E_CUDA; }
 extern "C" int ugvc_conc_classify(ugvc_conc*, int64_t, const int8_t*, const int8_t*, const uint8_t*, uint8_t*, uint8_t*) { return UGVC_E_CUDA; }

@@ -6,7 +6,7 @@ import pytest
 
 from oracle import concordance_ref as CR
 from tests.concordance_data import make_cases, make_frame
-from tests.test_concordance_cpu import check_accuracy, check_curve, load_golden
+from tests.test_concordance_cpu import assert_bits_equal, check_accuracy, check_curve, load_golden
 from variantcalling_b200 import concordance as PC
 
 pytestmark = pytest.mark.gpu
@@ -67,12 +67,14 @@ def test_evaluate_concordance_cli_writes_the_reference_csvs(tmp_path):
     df.to_csv(src, index=False)
     prefix = str(tmp_path / "out")
     EC.run(["--input_file", src, "--output_prefix", prefix])
-    stats = pd.read_csv(prefix + ".stats.csv", sep=";")
+    # the outputs hold shortest round-trip reprs: read them back exactly and compare bit for bit (the input is read
+    # as the CLI reads it)
+    stats = pd.read_csv(prefix + ".stats.csv", sep=";", float_precision="round_trip")
     want = CR.calc_accuracy_metrics(pd.read_csv(src), "classify_gt")
     assert list(stats.columns) == ["group"] + CR.METRIC_COLUMNS and list(stats["group"]) == list(want["group"])
     for col in CR.METRIC_COLUMNS:
-        np.testing.assert_allclose(stats[col].to_numpy(dtype=float), want[col].to_numpy(dtype=float), rtol=0, atol=1e-12)
-    thr = pd.read_csv(prefix + ".thresholds.csv")
+        assert_bits_equal(stats[col].to_numpy(dtype=float), want[col].to_numpy(dtype=float), col)
+    thr = pd.read_csv(prefix + ".thresholds.csv", float_precision="round_trip")
     want_thr = CR.calc_recall_precision_curve(pd.read_csv(src), "classify_gt")
     assert list(thr["group"]) == list(want_thr["group"])
-    np.testing.assert_allclose(thr["threshold"].to_numpy(dtype=float), np.asarray(list(want_thr["threshold"]), dtype=float))
+    assert_bits_equal(thr["threshold"].to_numpy(dtype=float), np.asarray(list(want_thr["threshold"]), dtype=float), "threshold")

@@ -28,7 +28,9 @@ from variantcalling_b200.multiallelics import read_fasta_contig
 
 logger = logging.getLogger(__name__)
 
-N_GROUPS, N_COUNTERS = 9, 6
+# ugvc_conc_run writes N_GROUPS x N_COUNTERS: the six metric counters (tp, fp, missed, initial_tp, n_called, n_fn),
+# then the NaN and +-inf scores among the called records
+N_GROUPS, N_COUNTERS, N_METRIC_COUNTERS = 9, 8, 6
 CLASS_CODE = {"fp": 0, "tp": 1, "fn": 2, "tn": 3}
 METRIC_COLUMNS = ["tp", "fp", "fn", "precision", "recall", "f1", "initial_tp", "initial_fp", "initial_fn",
                   "initial_precision", "initial_recall", "initial_f1"]
@@ -105,7 +107,8 @@ class ConcordanceContext:
         return int(self.lib.ugvc_conc_launch_count(self.h))
 
     def run(self, scores, pred, cls, indel, hmer, group=None, want_curves=True) -> dict:
-        """Arrays of one length -> dict(counts (9, 6), curve_len, cutoff, selected (9, 2))."""
+        """Arrays of one length -> dict(counts (9, 6), non_finite (9, 2): NaN / inf scores of called records,
+        curve_len, cutoff, selected (9, 2))."""
         n = len(scores)
         scores = np.ascontiguousarray(scores, dtype=np.float64)
         pred = np.ascontiguousarray(pred, dtype=np.uint8)
@@ -125,7 +128,8 @@ class ConcordanceContext:
                                     int(want_curves), p(counts), p(curve_len), p(cutoff), p(selected))
         if rc != 0:
             raise lib.UgvcError(rc, self.lib.ugvc_conc_last_error(self.h).decode())
-        return {"counts": counts, "curve_len": curve_len, "cutoff": cutoff, "selected": selected}
+        return {"counts": counts[:, :N_METRIC_COUNTERS].copy(), "non_finite": counts[:, N_METRIC_COUNTERS:].copy(),
+                "curve_len": curve_len, "cutoff": cutoff, "selected": selected}
 
     def classify(self, gt_ultima, gt_truth, base=None) -> tuple[np.ndarray, np.ndarray]:
         """The `classify` / `classify_gt` columns of vcf2concordance (comparison_utils.py:153-229) for genotype tuples
@@ -266,6 +270,26 @@ def _metrics_from_counts(c: np.ndarray) -> dict:
             "initial_recall": irecall, "initial_f1": get_f1(iprecision, irecall)}
 
 
+def _raise_on_non_finite(called_scores: np.ndarray, res: dict, groups, dtype) -> None:
+    """sklearn's assert_all_finite on the called scores of each group the reference draws a curve for (it draws one
+    even when only the metrics are returned), in its order: the first group with a NaN or an infinity raises, NaN's
+    message before inf's.  Whether any called score is non-finite is one pass over the host column; which group
+    meets it first comes from the device's per-group tallies.  dtype is the score column's, which sklearn names."""
+    if np.isfinite(called_scores).all():
+        return
+    for g in groups:
+        n_nan, n_inf = (int(v) for v in res["non_finite"][g])
+        if n_nan:
+            raise ValueError("Input contains NaN.")
+        if n_inf:
+            raise ValueError(f"Input contains infinity or a value too large for {dtype!r}.")
+
+
+def _score_dtype(scores) -> np.dtype:
+    dt = getattr(scores, "dtype", None)
+    return dt if dt is not None and dt.kind == "f" else np.dtype(np.float64)
+
+
 def _curve_from_device(ctx: ConcordanceContext, g: int, res: dict) -> dict:
     """stats_utils.precision_recall_curve :141-210 after the sklearn call, and the threshold choice of
     get_concordance_metrics :391-407, from the raw device curve of group g."""
@@ -279,7 +303,8 @@ def _curve_from_device(ctx: ConcordanceContext, g: int, res: dict) -> dict:
         return {"threshold": 0, "predictions": [], "precision": [], "recall": [], "f1": []}
     raw_p, raw_r, thr = ctx.curve(g, int(res["curve_len"][g]))
     sel_true = int(res["selected"][g, 1])
-    correction = sel_true / (sel_true + n_fn)
+    with np.errstate(invalid="ignore"):  # no true call and no false negative: NaN recalls, as NumPy gives the reference
+        correction = np.float64(sel_true) / np.float64(sel_true + n_fn)
     # sklearn appends (1, 0) to precision / recall; the reference then drops the first and last points
     recalls = (np.hstack((raw_r, 0)) * correction)[1:-1]
     precisions = np.hstack((raw_p, 1))[1:-1]
@@ -302,6 +327,8 @@ def get_concordance_metrics(predictions, scores, truth, fn_mask, *, return_metri
     n = len(cls)
     res = ctx.run(scores, np.asarray(predictions) > 0, cls, np.zeros(n, np.uint8), np.zeros(n, np.int32),
                   group=np.zeros(n, np.int8), want_curves=return_curves)
+    scores = np.asarray(scores)
+    _raise_on_non_finite(np.asarray(scores[~fn_mask], dtype=np.float64), res, [0], _score_dtype(scores))
     metrics_df = pd.DataFrame(_metrics_from_counts(res["counts"][0]), index=[0])
     if not return_curves:
         return metrics_df
@@ -346,8 +373,12 @@ def _device_pass(concordance_df, classify_column_name, group_testing_column_name
         ids = {name: i for i, name in enumerate(GROUP_NAMES)}
         group = df["group_testing"].map(lambda v: ids.get(v, -1)).to_numpy(dtype=np.int8)
     ctx = _context(ctx)
-    res = ctx.run(df["tree_score"].to_numpy(dtype=np.float64), pred, cls, df["indel"].to_numpy(dtype=bool), hmer,
-                  group=group, want_curves=want_curves)
+    scores = df["tree_score"].to_numpy(dtype=np.float64)
+    res = ctx.run(scores, pred, cls, df["indel"].to_numpy(dtype=bool), hmer, group=group, want_curves=want_curves)
+    # calc_accuracy_metrics draws the curves of the 7 groups, INDELS and H-INDELS; calc_recall_precision_curve of
+    # all but H-INDELS
+    _raise_on_non_finite(scores[cls != CLASS_CODE["fn"]], res, range(N_GROUPS - 1) if want_curves else range(N_GROUPS),
+                         _score_dtype(df["tree_score"]))
     return ctx, res
 
 

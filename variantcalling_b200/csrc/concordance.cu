@@ -9,8 +9,10 @@
 // The host mirror (variantcalling_b200/concordance.py) keeps the reference's function signatures and
 // does the O(#groups) arithmetic; everything that touches N records runs here:
 //   C1 conc_classify   one pass over the records: group membership, truth / call bits, and the
-//                      9 x 6 counters (block-local shared-memory atomics, one global atomic per counter
-//                      per block).  HBM-bound: 15 B read + 3 B written per record.
+//                      9 x 8 counters (block-local shared-memory atomics, one global atomic per counter
+//                      per block), NaN / inf scores of called records among them.  A group id outside
+//                      -1..6 or a class code above 3 flags the call and counts nothing.  HBM-bound:
+//                      23 B read + 3 B written per record.
 //   per group g with a curve:
 //   C2 conc_flags      membership & not-false-negative flag
 //      cub::DeviceSelect::Flagged          scores / truth of the group, compacted
@@ -19,7 +21,10 @@
 //   C3 conc_boundary   last element of every run of equal scores (np.diff(score) != 0)
 //      cub::DeviceSelect::Flagged          their indices
 //   C4 conc_curve      precision = tps / (tps + fps), recall = tps / tps[-1] in fp64 (IEEE division, the
-//                      same bits as NumPy), written in increasing-threshold order like sklearn returns them
+//                      same bits as NumPy), written in increasing-threshold order like sklearn returns them;
+//                      the threshold of a run is its first element (the radix sort is stable and ranks
+//                      -0.0 with +0.0, so that is the run's first score in input order, as the pinned
+//                      scikit-learn 1.5 reports it: a run of signed zeros keeps its first zero's sign)
 #include <cub/cub.cuh>
 
 #include <algorithm>
@@ -38,14 +43,18 @@ __global__ void __launch_bounds__(CONC_TPB) conc_classify(int64_t n, const uint8
                                                            const int32_t* __restrict__ hmer,
                                                            const int8_t* __restrict__ group, uint16_t* __restrict__ meta,
                                                            uint8_t* __restrict__ truth8,
+                                                           const double* __restrict__ scores,
                                                            unsigned long long* __restrict__ counts) {
     __shared__ unsigned int s_cnt[CONC_GROUPS * CONC_COUNTERS];
+    __shared__ unsigned int s_bad;
     for (int i = threadIdx.x; i < CONC_GROUPS * CONC_COUNTERS; i += CONC_TPB) s_cnt[i] = 0u;
+    if (threadIdx.x == 0) s_bad = 0u;
     __syncthreads();
     const int64_t stride = (int64_t)gridDim.x * CONC_TPB;
     for (int64_t i = (int64_t)blockIdx.x * CONC_TPB + threadIdx.x; i < n; i += stride) {
         const bool ind = indel[i] != 0;
         const int h = hmer[i];
+        const unsigned c = cls[i];  // 0 fp, 1 tp, 2 fn, 3 tn
         int gid;
         if (group) {
             gid = group[i];
@@ -58,8 +67,14 @@ __global__ void __launch_bounds__(CONC_TPB) conc_classify(int64_t n, const uint8
         } else {
             gid = h <= 4 ? 2 : h <= 7 ? 3 : h <= 10 ? 4 : h <= 12 ? 5 : 6;
         }
-        const unsigned c = cls[i];  // 0 fp, 1 tp, 2 fn, 3 tn
+        if (gid < -1 || gid >= 7 || c > 3u) {  // outside the ABI: refused by the host, never used as an index
+            s_bad = 1u;
+            continue;
+        }
         const bool truth = c == 1u || c == 2u, fnm = c == 2u, call = pred[i] != 0;
+        // sklearn's assert_all_finite on the scores of the called records (the false negatives are dropped first)
+        const double sc = fnm ? 0.0 : scores[i];
+        const bool s_nan = isnan(sc), s_inf = isinf(sc);
         const unsigned m = (unsigned)(gid + 1) | (truth ? 16u : 0u) | (fnm ? 32u : 0u) | (call ? 64u : 0u) |
                            (ind ? 128u : 0u) | (h > 0 ? 256u : 0u);
         meta[i] = (uint16_t)m;
@@ -77,12 +92,15 @@ __global__ void __launch_bounds__(CONC_TPB) conc_classify(int64_t n, const uint8
                 if (truth && call) atomicAdd(cg + 0, 1u);
                 if (call && !truth) atomicAdd(cg + 1, 1u);
                 if (!call && truth) atomicAdd(cg + 2, 1u);
+                if (s_nan) atomicAdd(cg + 6, 1u);
+                if (s_inf) atomicAdd(cg + 7, 1u);
             }
         }
     }
     __syncthreads();
     for (int i = threadIdx.x; i < CONC_GROUPS * CONC_COUNTERS; i += CONC_TPB)
         if (s_cnt[i]) atomicAdd(counts + i, (unsigned long long)s_cnt[i]);
+    if (threadIdx.x == 0 && s_bad) atomicAdd(counts + CONC_GROUPS * CONC_COUNTERS, 1ull);
 }
 
 __global__ void __launch_bounds__(CONC_TPB) conc_flags(int64_t n, const uint16_t* __restrict__ meta, int g,
@@ -115,7 +133,7 @@ __global__ void __launch_bounds__(CONC_TPB) conc_curve(int64_t d, int64_t n_sel,
         const int64_t o = d - 1 - k;
         out_p[o] = ps != 0.0 ? __ddiv_rn(tps, ps) : 0.0;
         out_r[o] = total == 0.0 ? 1.0 : __ddiv_rn(tps, total);
-        out_t[o] = s[at];
+        out_t[o] = s[k == 0 ? 0 : idx[k - 1] + 1];
     }
 }
 
@@ -187,15 +205,19 @@ extern "C" int ugvc_conc_run(ugvc_conc* h, int64_t n, const double* scores, cons
     CCU(buf.get(&d_meta, (size_t)n));
     CCU(buf.get(&d_truth, (size_t)n));
     CCU(buf.get(&d_flags, (size_t)n));
-    CCU(buf.get(&d_counts, (size_t)CONC_GROUPS * CONC_COUNTERS));
-    CCU(cudaMemsetAsync(d_counts, 0, sizeof(unsigned long long) * CONC_GROUPS * CONC_COUNTERS, st));
+    // the counters, then one slot for the blocks that met a record outside the ABI
+    CCU(buf.get(&d_counts, (size_t)CONC_GROUPS * CONC_COUNTERS + 1));
+    CCU(cudaMemsetAsync(d_counts, 0, sizeof(unsigned long long) * (CONC_GROUPS * CONC_COUNTERS + 1), st));
     const int grid = h->sm_count * 8;
-    conc_classify<<<grid, CONC_TPB, 0, st>>>(n, d_pred, d_cls, d_indel, d_hmer, d_group, d_meta, d_truth, d_counts);
+    conc_classify<<<grid, CONC_TPB, 0, st>>>(n, d_pred, d_cls, d_indel, d_hmer, d_group, d_meta, d_truth, d_scores,
+                                             d_counts);
     ++h->launches;
     CCU(cudaGetLastError());
-    unsigned long long h_counts[CONC_GROUPS * CONC_COUNTERS];
+    unsigned long long h_counts[CONC_GROUPS * CONC_COUNTERS + 1];
     CCU(cudaMemcpyAsync(h_counts, d_counts, sizeof(h_counts), cudaMemcpyDeviceToHost, st));
     CCU(cudaStreamSynchronize(st));
+    if (h_counts[CONC_GROUPS * CONC_COUNTERS])
+        return conc_fail(h, UGVC_E_ARG, "conc_run: a group id outside -1..6 or a class code above 3");
     for (int i = 0; i < CONC_GROUPS * CONC_COUNTERS; ++i) out_counts[i] = (int64_t)h_counts[i];
     if (!want_curves) return UGVC_OK;
 

@@ -10,7 +10,7 @@
 #include "../../include/ugvc_b200.h"
 
 #define CONC_GROUPS UGVC_CONC_GROUPS      // 7 default groups + INDELS + H-INDELS
-#define CONC_COUNTERS UGVC_CONC_COUNTERS  // tp, fp, missed (call < truth), initial_tp, n_called, n_fn
+#define CONC_COUNTERS UGVC_CONC_COUNTERS  // tp, fp, missed (call < truth), initial_tp, n_called, n_fn, n_nan, n_inf
 #define CONC_TPB 256
 
 struct ugvc_conc {

@@ -130,6 +130,7 @@ SIGNATURES = {
     "ugvc_conc_free": (None, [_vp]),
     "ugvc_conc_last_error": (C.c_char_p, [_vp]),
     "ugvc_conc_launch_count": (C.c_longlong, [_vp]),
+    # out_counts: int64[9][8] (UGVC_CONC_GROUPS x UGVC_CONC_COUNTERS, the last two: NaN / inf scores of called records)
     "ugvc_conc_run": (C.c_int, [_vp, C.c_int64, _vp, _vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int, _vp, _vp, _vp, _vp]),
     "ugvc_conc_classify": (C.c_int, [_vp, C.c_int64, _vp, _vp, _vp, _vp, _vp]),
     "ugvc_conc_curve": (C.c_int, [_vp, C.c_int, _vp, _vp, _vp, _sz]),
