@@ -597,6 +597,62 @@ int64_t ugvc_test_bsn(const uint8_t* text, size_t n_bytes, const int64_t* line_s
                       uint8_t* out_rescued, int32_t* out_hmer, int64_t* out_end, int64_t* out_n_rescued,
                       int64_t* out_err_record, int32_t* out_err_reason);
 
+/* ---- gvcf_hcr on the device (DESIGN.md 4e) ---------------------------------
+ * Replaces ugvc/joint/gvcf_bed.py:gvcf_to_bed and the bedtools merge of ugvc/pipelines/vcfbed/gvcf_hcr_main.py: each
+ * record's interval [POS - 1, end) (end = INFO/END under the index rule, else POS - 1 + len(REF); a RefCall deletion --
+ * len(REF) > 1 and sample 0 without GQ, or with GT (0, 0) or (None, None) -- ends at POS), records that start before the
+ * end of the last kept record of their contig skipped, kept records selected by sample 0's GQ (gt: GQ >= threshold,
+ * else GQ absent or < threshold) and written as BED lines "CHROM\tstart\tend\n" (merge: book-ended selected records
+ * joined into one line).  The output is plain text. */
+#define UGVC_HCR_GQ_STRING 0   /* GQ undeclared or of Type String / Character: comparing it raises TypeError */
+#define UGVC_HCR_GQ_SCALAR 1   /* Number=1, Integer or Float */
+#define UGVC_HCR_GQ_TUPLE 2    /* any other Number: comparing it raises TypeError */
+#define UGVC_HCR_E_LITERAL 1   /* a GQ / GT literal the parser refuses (numparse.h) */
+#define UGVC_HCR_E_TYPE 2      /* TypeError: a kept record's GQ is None, a tuple or a string */
+#define UGVC_HCR_E_KEY 3       /* KeyError: a RefCall candidate whose FORMAT has GQ but not GT */
+#define UGVC_HCR_E_UNSORTED 4  /* POS decreases within a contig: the file cannot carry a tabix index */
+#define UGVC_HCR_SELECTED 1    /* flags: selected if the record is kept */
+#define UGVC_HCR_GQ_ERROR 2    /* flags: comparing the record's GQ raises TypeError */
+#define UGVC_HCR_NEW_CONTIG 4  /* flags: the record starts a contig run of the call */
+#define UGVC_HCR_RESET 8       /* flags: the record starts at or after every earlier end of its contig (kept for sure) */
+#define UGVC_HCR_KEPT 16       /* flags: not skipped */
+#define UGVC_HCR_LINE 32       /* flags: the record starts an output line */
+typedef struct ugvc_hcr_params {
+    int64_t gq_threshold;
+    int32_t gt;          /* 1: GQ >= threshold; 0: GQ absent or GQ < threshold */
+    int32_t merge;       /* 1: one line per merged (book-ended) run of selected records; 0: one per selected record */
+    int32_t info_end;    /* the header declares INFO/END */
+    int32_t gq_kind;     /* UGVC_HCR_GQ_*: how the header declares FORMAT/GQ */
+    int32_t gq_integer;  /* Type=Integer (else Float) */
+} ugvc_hcr_params;
+/* First half of one range of whole gVCF data lines (BGZF blocks, skip_head / take_bytes as for ugvc_afr_bgzf): inflate,
+ * the index K1 pass of the model-less plan, then per record the interval, the selection and the GQ / GT checks, and the
+ * per-contig prefix maximum of the ends.  The piece stays on the lane for ugvc_hcr_emit.  out_stats = {contig runs that
+ * start in the range, the first record > 0 that starts one (n: none), POS - 1 of the first and of the last record};
+ * out_run_starts (2 * capacity_records entries) a (record, line start) pair for each record that starts a contig run,
+ * in no order. */
+int ugvc_hcr_scan(ugvc_ctx* ctx, int lane, const uint8_t* data, size_t n_bytes, uint32_t skip_head, uint64_t take_bytes,
+                  const ugvc_hcr_params* params, size_t capacity_records, int64_t* out_n_records, int64_t out_stats[4],
+                  int64_t* out_run_starts);
+/* Second half, in file order: the kept flags from the entry state (continues_contig: the range's first record is on the
+ * contig of the previous range's last one, whose kept records end at entry_extent), selection, merge and the BED text
+ * (*out_bytes bytes at out_bed).  out_stats = {output lines, skipped records, the exit extent (end of the last kept
+ * record; entry_extent or -1 when none), longest reset-to-reset segment}.  UGVC_E_DATA where the reference raises:
+ * ugvc_hcr_error gives the record (index in the range) and the UGVC_HCR_E_* reason. */
+int ugvc_hcr_emit(ugvc_ctx* ctx, int lane, const ugvc_hcr_params* params, int continues_contig, int64_t entry_extent,
+                  uint8_t* out_bed, size_t out_capacity, size_t* out_bytes, int64_t out_stats[4]);
+int ugvc_hcr_error(const ugvc_ctx* ctx, int lane, int64_t* out_record, int32_t* out_reason);
+/* ms of the last scan + emit on `lane` between CUDA events: H2D + inflate, index K1, decide + prefix max, emit kernels,
+ * D2H. */
+int ugvc_hcr_stage_ms(ugvc_ctx* ctx, int lane, float out_ms[5]);
+/* Test hook: scan and emit kernels on the caller's records (line_start: n + 1 entries, every line ending with '\n') with
+ * the given entry state, without a context.  seg_bound: records a thread walks before a segment takes the parallel form
+ * (0: the build's bound).  out_flags (n bytes) the UGVC_HCR_* flags, out_stats as ugvc_hcr_emit's.  Returns the bytes
+ * written to out, UGVC_E_DATA with *out_err_record / *out_err_reason where the reference raises. */
+int64_t ugvc_test_hcr(const uint8_t* text, size_t n_bytes, const int64_t* line_start, int64_t n, const ugvc_hcr_params* params,
+                      int continues_contig, int64_t entry_extent, int64_t seg_bound, uint8_t* out, size_t capacity,
+                      uint8_t* out_flags, int64_t out_stats[4], int64_t* out_err_record, int32_t* out_err_reason);
+
 /* ---- test hook ------------------------------------------------------------ */
 /* K1's numeric-literal parser (csrc/numparse.h) compiled for the host: parses one token of
  * `text` (NUL-terminated); returns 0 ok / 1 missing (".") / 2 not exactly parseable. */

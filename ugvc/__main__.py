@@ -16,6 +16,7 @@ if ROOT not in sys.path:
 TOOLS = {"filter_variants_pipeline": "variantcalling_b200.filter_variants_pipeline",
          "filter_low_af_ratio_to_background": "variantcalling_b200.low_af_ratio",
          "calibrate_bridging_snvs": "variantcalling_b200.bridging_snvs",
+         "gvcf_hcr": "variantcalling_b200.gvcf_hcr",
          "evaluate_concordance": "variantcalling_b200.evaluate_concordance"}
 
 

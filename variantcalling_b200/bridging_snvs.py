@@ -206,28 +206,13 @@ def calibrate_bridging_snvs(
         except lib.UgvcDataError as err:
             if getattr(err, "bsn_record", -1) < 0:
                 raise
-            line = _line_at(src, src.starts[done], err.bsn_record)
+            line = src.line_at(src.starts[done], err.bsn_record)
             _raise_for(err, first + err.bsn_record, line, params.min_query_hmer_size)
         writer.close()
         index.write(final + ".tbi")
     finally:
         ctx.close()
     return n_rescued
-
-
-def _line_at(src: vcf_pieces.Input, u0: int, r: int) -> str:
-    """Data line r of the piece that starts at uncompressed offset u0 (read back from the input)."""
-    at, chunk = u0, b""
-    for _ in range(r + 1):
-        at += len(chunk)
-        chunk = src.text(at, at + (1 << 16))
-        while b"\n" not in chunk:
-            more = src.text(at + len(chunk), at + len(chunk) + (1 << 16))
-            if not more:
-                break
-            chunk += more
-        chunk = chunk[: chunk.find(b"\n") + 1] if b"\n" in chunk else chunk
-    return chunk.rstrip(b"\n").decode("latin-1")
 
 
 def _log_rescued(src: vcf_pieces.Input, u0: int, res: dict, contigs: dict, m: int):

@@ -15,6 +15,7 @@
 #include "fileio.cuh"
 #include "low_af_ratio.cuh"
 #include "bridging_snvs.cuh"
+#include "gvcf_hcr.cuh"
 #include "multiallelic.cuh"
 #endif
 
@@ -85,6 +86,15 @@ struct Lane {
         float ms_bsn[5] = {0, 0, 0, 0, 0};
         int64_t bsn_err_record = -1;
         int32_t bsn_err_reason = 0;
+#ifndef UGVC_HOST_EMU
+        // ugvc_hcr_scan / ugvc_hcr_emit: the piece's records between the two calls, events of the decide and the emit
+        HcrBufs hcr;
+        cudaEvent_t ev_hcr[4] = {nullptr, nullptr, nullptr, nullptr};
+        float ms_hcr[5] = {0, 0, 0, 0, 0};
+        bool hcr_scanned = false;
+        int64_t hcr_err_record = -1;
+        int32_t hcr_err_reason = 0;
+#endif
     } fb;
 };
 
@@ -218,6 +228,11 @@ static void free_lane(Lane& l) {
     cudaFree(l.fb.d_afr_tot);
     if (l.fb.h_afr_tot) cudaFreeHost(l.fb.h_afr_tot);
     cudaFree(l.fb.d_bsn_hmer);
+#ifndef UGVC_HOST_EMU
+    hcr_bufs_free(&l.fb.hcr);
+    for (auto& e : l.fb.ev_hcr)
+        if (e) cudaEventDestroy(e);
+#endif
     for (auto& e : l.fb.ev)
         if (e) cudaEventDestroy(e);
     for (auto& e : l.fb.ev_split)
@@ -1414,6 +1429,15 @@ extern "C" int ugvc_bsn_bgzf(ugvc_ctx* ctx, int, const uint8_t*, size_t, uint32_
 }
 extern "C" int ugvc_bsn_error(const ugvc_ctx*, int, int64_t*, int32_t*) { return UGVC_E_STATE; }
 extern "C" int ugvc_bsn_stage_ms(ugvc_ctx*, int, float*) { return UGVC_E_STATE; }
+extern "C" int ugvc_hcr_scan(ugvc_ctx* ctx, int, const uint8_t*, size_t, uint32_t, uint64_t, const ugvc_hcr_params*, size_t, int64_t*,
+                             int64_t*, int64_t*) {
+    return fail(ctx, UGVC_E_STATE, "the device file path of gvcf_hcr is not part of the host emulation");
+}
+extern "C" int ugvc_hcr_emit(ugvc_ctx* ctx, int, const ugvc_hcr_params*, int, int64_t, uint8_t*, size_t, size_t*, int64_t*) {
+    return fail(ctx, UGVC_E_STATE, "the device file path of gvcf_hcr is not part of the host emulation");
+}
+extern "C" int ugvc_hcr_error(const ugvc_ctx*, int, int64_t*, int32_t*) { return UGVC_E_STATE; }
+extern "C" int ugvc_hcr_stage_ms(ugvc_ctx*, int, float*) { return UGVC_E_STATE; }
 #else
 #define FIO_BL_NAMES_AT (8 * (UGVC_MAX_BLACKLISTS + 1) + 4 * (UGVC_MAX_BLACKLISTS + 2))
 #define FIO_BL_META (FIO_BL_NAMES_AT + UGVC_MAX_BLACKLIST_NAME_BYTES)
@@ -2300,6 +2324,101 @@ extern "C" int ugvc_bsn_error(const ugvc_ctx* ctx, int lane, int64_t* out_record
 extern "C" int ugvc_bsn_stage_ms(ugvc_ctx* ctx, int lane, float out_ms[5]) {
     if (!ctx || lane < 0 || lane >= (int)ctx->lanes.size() || !out_ms) return UGVC_E_ARG;
     memcpy(out_ms, ctx->lanes[lane].fb.ms_bsn, sizeof(ctx->lanes[lane].fb.ms_bsn));
+    return UGVC_OK;
+}
+
+// ---- gvcf_hcr: the scan (inflate, index K1, decide, prefix max) on both lanes, the emit in piece order
+extern "C" int ugvc_hcr_scan(ugvc_ctx* ctx, int lane, const uint8_t* data, size_t n_bytes, uint32_t skip_head, uint64_t take_bytes,
+                             const ugvc_hcr_params* params, size_t capacity_records, int64_t* out_n_records, int64_t out_stats[4],
+                             int64_t* out_run_starts) {
+    if (!ctx) return UGVC_E_ARG;
+    HcrDev P;
+    if (!hcr_params(params, &P)) return fail(ctx, UGVC_E_ARG, "hcr_scan: bad params");
+    if (!ctx->has_plan || ctx->lanes.empty()) return fail(ctx, UGVC_E_STATE, "hcr_scan: load the model-less plan and reserve first");
+    if (lane < 0 || lane >= (int)ctx->lanes.size()) return fail(ctx, UGVC_E_ARG, "hcr_scan: lane out of range");
+    if (!data || !n_bytes || !out_n_records || !out_stats || !out_run_starts) return fail(ctx, UGVC_E_ARG, "hcr_scan: bad argument");
+    CU(cudaSetDevice(ctx->device));
+    Lane& l = ctx->lanes[lane];
+    if (l.submitted) return fail(ctx, UGVC_E_STATE, "hcr_scan: lane already has a batch in flight");
+    Lane::FileBufs& f = l.fb;
+    f.hcr_scanned = false;
+    const uint8_t* d_text = nullptr;
+    int64_t n = 0;
+    int rc = tool_front(ctx, l, "hcr_scan", data, n_bytes, skip_head, take_bytes, 0, capacity_records, &d_text, &n);
+    *out_n_records = n;
+    if (rc) return rc;
+    cudaStream_t st = l.stream;
+    if (!f.ev_hcr[0])
+        for (auto& e : f.ev_hcr) CU(cudaEventCreate(&e));
+    CU(hcr_bufs_reserve(&f.hcr, l.b.cap_records));
+    hcr_launch_scan(d_text, l.b.line_start, n, P, &f.hcr, ctx->sm_count, st);
+    CU(cudaGetLastError());
+    CU(cudaEventRecord(f.ev_hcr[0], st));
+    int64_t stat[HCR_STAT_N];
+    CU(cudaMemcpyAsync(stat, f.hcr.stat, sizeof(stat), cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    const int64_t n_runs = stat[HCR_STAT_N_RUNS];
+    if (n_runs) CU(cudaMemcpy(out_run_starts, f.hcr.runs, 2 * (size_t)n_runs * sizeof(int64_t), cudaMemcpyDeviceToHost));
+    out_stats[0] = n_runs;
+    out_stats[1] = stat[HCR_STAT_R0];
+    out_stats[2] = stat[HCR_STAT_FIRST_START];
+    out_stats[3] = stat[HCR_STAT_LAST_START];
+    f.hcr_scanned = true;
+    return UGVC_OK;
+}
+
+extern "C" int ugvc_hcr_emit(ugvc_ctx* ctx, int lane, const ugvc_hcr_params* params, int continues_contig, int64_t entry_extent,
+                             uint8_t* out_bed, size_t out_capacity, size_t* out_bytes, int64_t out_stats[4]) {
+    if (!ctx) return UGVC_E_ARG;
+    HcrDev P;
+    if (!hcr_params(params, &P)) return fail(ctx, UGVC_E_ARG, "hcr_emit: bad params");
+    if (lane < 0 || lane >= (int)ctx->lanes.size()) return fail(ctx, UGVC_E_ARG, "hcr_emit: lane out of range");
+    if (!out_bytes || !out_stats) return fail(ctx, UGVC_E_ARG, "hcr_emit: bad argument");
+    CU(cudaSetDevice(ctx->device));
+    Lane& l = ctx->lanes[lane];
+    Lane::FileBufs& f = l.fb;
+    if (!f.hcr_scanned) return fail(ctx, UGVC_E_STATE, "hcr_emit: no scanned piece on the lane");
+    f.hcr_scanned = false;
+    f.hcr_err_record = -1;
+    f.hcr_err_reason = 0;
+    cudaStream_t st = l.stream;
+    CU(cudaEventRecord(f.ev_hcr[1], st));
+    HcrEmitOut r{};
+    CU(hcr_emit(&f.hcr, P, continues_contig, entry_extent, HCR_SEG_BOUND, f.d_out_text, f.cap_out, &r, ctx->sm_count, st));
+    CU(cudaEventRecord(f.ev_hcr[2], st));
+    out_stats[0] = r.n_lines;
+    out_stats[1] = r.skipped;
+    out_stats[2] = r.exit_extent;
+    out_stats[3] = r.longest;
+    if ((unsigned long long)r.err != AFR_NO_ERROR) {
+        f.hcr_err_record = (int64_t)((unsigned long long)r.err >> 4);
+        f.hcr_err_reason = (int32_t)((unsigned long long)r.err & 0xF);
+        return fail(ctx, UGVC_E_DATA, "hcr_emit: the reference raises at record " + std::to_string(f.hcr_err_record) + " (reason " +
+                                          std::to_string(f.hcr_err_reason) + ")");
+    }
+    if ((size_t)r.bytes > out_capacity || (r.bytes && !out_bed)) return fail(ctx, UGVC_E_ARG, "hcr_emit: out_capacity smaller than the BED text");
+    if (r.bytes) CU(cudaMemcpyAsync(out_bed, f.d_out_text, (size_t)r.bytes, cudaMemcpyDeviceToHost, st));
+    CU(cudaEventRecord(f.ev_hcr[3], st));
+    CU(cudaStreamSynchronize(st));
+    *out_bytes = (size_t)r.bytes;
+    cudaEventElapsedTime(&f.ms_hcr[0], f.ev[0], f.ev[1]);
+    cudaEventElapsedTime(&f.ms_hcr[1], f.ev[1], f.ev[2]);
+    cudaEventElapsedTime(&f.ms_hcr[2], f.ev[2], f.ev_hcr[0]);
+    cudaEventElapsedTime(&f.ms_hcr[3], f.ev_hcr[1], f.ev_hcr[2]);
+    cudaEventElapsedTime(&f.ms_hcr[4], f.ev_hcr[2], f.ev_hcr[3]);
+    return UGVC_OK;
+}
+
+extern "C" int ugvc_hcr_error(const ugvc_ctx* ctx, int lane, int64_t* out_record, int32_t* out_reason) {
+    if (!ctx || lane < 0 || lane >= (int)ctx->lanes.size() || !out_record || !out_reason) return UGVC_E_ARG;
+    *out_record = ctx->lanes[lane].fb.hcr_err_record;
+    *out_reason = ctx->lanes[lane].fb.hcr_err_reason;
+    return UGVC_OK;
+}
+
+extern "C" int ugvc_hcr_stage_ms(ugvc_ctx* ctx, int lane, float out_ms[5]) {
+    if (!ctx || lane < 0 || lane >= (int)ctx->lanes.size() || !out_ms) return UGVC_E_ARG;
+    memcpy(out_ms, ctx->lanes[lane].fb.ms_hcr, sizeof(ctx->lanes[lane].fb.ms_hcr));
     return UGVC_OK;
 }
 #endif  // !UGVC_HOST_EMU

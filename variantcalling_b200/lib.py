@@ -70,6 +70,17 @@ BSN_RESCUED, BSN_NEW_CONTIG = 1, 4
 BSN_MAX_QUAL_BYTES = 31
 
 
+class HcrParams(C.Structure):
+    """ugvc_hcr_params (include/ugvc_b200.h)."""
+    _fields_ = [("gq_threshold", C.c_int64), ("gt", C.c_int32), ("merge", C.c_int32), ("info_end", C.c_int32),
+                ("gq_kind", C.c_int32), ("gq_integer", C.c_int32)]
+
+
+HCR_GQ_STRING, HCR_GQ_SCALAR, HCR_GQ_TUPLE = 0, 1, 2
+HCR_E_LITERAL, HCR_E_TYPE, HCR_E_KEY, HCR_E_UNSORTED = 1, 2, 3, 4
+HCR_SELECTED, HCR_GQ_ERROR, HCR_NEW_CONTIG, HCR_RESET, HCR_KEPT, HCR_LINE = 1, 2, 4, 8, 16, 32
+
+
 class Counts(C.Structure):
     _fields_ = [("n_records", C.c_int64), ("n_low_score", C.c_int64), ("n_pass", C.c_int64), ("n_cg", C.c_int64)]
 
@@ -189,6 +200,12 @@ SIGNATURES = {
     "ugvc_bsn_stage_ms": (C.c_int, [_vp, C.c_int, _vp]),
     "ugvc_test_bsn": (C.c_int64, [_vp, _sz, _vp, C.c_int64, _vp, _vp, _vp, _vp, C.c_int32, C.POINTER(BsnParams), _vp, _sz,
                                   _vp, _vp, _vp, _vp, _i64p, _i64p, C.POINTER(C.c_int32)]),
+    "ugvc_hcr_scan": (C.c_int, [_vp, C.c_int, _vp, _sz, C.c_uint32, C.c_uint64, C.POINTER(HcrParams), _sz, _i64p, _vp, _vp]),
+    "ugvc_hcr_emit": (C.c_int, [_vp, C.c_int, C.POINTER(HcrParams), C.c_int, C.c_int64, _vp, _sz, C.POINTER(_sz), _vp]),
+    "ugvc_hcr_error": (C.c_int, [_vp, C.c_int, _i64p, C.POINTER(C.c_int32)]),
+    "ugvc_hcr_stage_ms": (C.c_int, [_vp, C.c_int, _vp]),
+    "ugvc_test_hcr": (C.c_int64, [_vp, _sz, _vp, C.c_int64, C.POINTER(HcrParams), C.c_int, C.c_int64, C.c_int64, _vp, _sz,
+                                  _vp, _vp, _i64p, C.POINTER(C.c_int32)]),
 }
 
 # the concordance-frame annotation entry points are bound on first use (load_annotation), so that a build of the
@@ -198,11 +215,14 @@ _BOUND_ON_USE = frozenset(n for n in SIGNATURES if n.startswith("ugvc_conc_annot
 _AFR_BOUND_ON_USE = frozenset(n for n in SIGNATURES if n.startswith(("ugvc_afr_", "ugvc_test_afr")))
 # and those of calibrate_bridging_snvs (load_bridging_snvs)
 _BSN_BOUND_ON_USE = frozenset(n for n in SIGNATURES if n.startswith(("ugvc_bsn_", "ugvc_test_bsn")))
+# and those of gvcf_hcr (load_gvcf_hcr)
+_HCR_BOUND_ON_USE = frozenset(n for n in SIGNATURES if n.startswith(("ugvc_hcr_", "ugvc_test_hcr")))
 
 _lib = None
 _annotation_bound = False
 _afr_bound = False
 _bsn_bound = False
+_hcr_bound = False
 
 
 def load_library() -> C.CDLL:
@@ -215,7 +235,7 @@ def load_library() -> C.CDLL:
                 f"(make -C variantcalling_b200/csrc).  There is no CPU fallback for the hot path.")
         lib = C.CDLL(LIB_PATH)
         for name, (res, args) in SIGNATURES.items():
-            if name in _BOUND_ON_USE or name in _AFR_BOUND_ON_USE or name in _BSN_BOUND_ON_USE:
+            if name in _BOUND_ON_USE or name in _AFR_BOUND_ON_USE or name in _BSN_BOUND_ON_USE or name in _HCR_BOUND_ON_USE:
                 continue
             fn = getattr(lib, name)
             fn.restype = res
@@ -263,6 +283,20 @@ def load_bridging_snvs() -> C.CDLL:
             fn.restype = res
             fn.argtypes = args
         _bsn_bound = True
+    return lib
+
+
+def load_gvcf_hcr() -> C.CDLL:
+    """load_library() with the gvcf_hcr entry points bound.  Raises if the library lacks them."""
+    global _hcr_bound  # noqa: PLW0603
+    lib = load_library()
+    if not _hcr_bound:
+        for name in sorted(_HCR_BOUND_ON_USE):
+            res, args = SIGNATURES[name]
+            fn = getattr(lib, name)
+            fn.restype = res
+            fn.argtypes = args
+        _hcr_bound = True
     return lib
 
 
@@ -658,6 +692,48 @@ class Context:
         self._check(load_bridging_snvs().ugvc_bsn_stage_ms(self.h, lane, C.cast(ms, C.c_void_p)))
         return list(ms)
 
+    def hcr_scan(self, data: np.ndarray, skip_head: int, take_bytes: int, params: HcrParams, max_records: int,
+                 lane: int = 0) -> dict:
+        """The first half of gvcf_hcr on one range of whole lines of BGZF blocks (ugvc_hcr_scan): inflate, index, decide
+        and the per-contig prefix max; the piece stays on the lane for hcr_emit.  {"n_records", "runs" ((record, line
+        start) of each record that starts a contig run, by record), "r0", "first_start", "last_start"}."""
+        lib = load_gvcf_hcr()
+        src = np.ascontiguousarray(data, dtype=np.uint8)
+        runs = np.empty((max(1, max_records), 2), dtype=np.int64)
+        stats = np.zeros(4, dtype=np.int64)
+        n = C.c_int64()
+        self._check(lib.ugvc_hcr_scan(self.h, lane, _ptr(src), src.size, skip_head, take_bytes, C.byref(params), max_records,
+                                      C.byref(n), _ptr(stats), _ptr(runs)))
+        runs = runs[: int(stats[0])]
+        return {"n_records": n.value, "runs": runs[np.argsort(runs[:, 0])], "r0": int(stats[1]),
+                "first_start": int(stats[2]), "last_start": int(stats[3])}
+
+    def hcr_emit(self, params: HcrParams, continues_contig: bool, entry_extent: int, capacity: int, lane: int = 0) -> dict:
+        """The second half (ugvc_hcr_emit) on the piece `lane` holds: {"bed" (bytes), "n_lines", "skipped",
+        "exit_extent", "longest_segment"}.  A record the reference raises at comes back as UgvcDataError with
+        .hcr_record / .hcr_reason set."""
+        lib = load_gvcf_hcr()
+        out = np.empty(max(1, capacity), dtype=np.uint8)
+        stats = np.zeros(4, dtype=np.int64)
+        nb = C.c_size_t()
+        rc = lib.ugvc_hcr_emit(self.h, lane, C.byref(params), int(bool(continues_contig)), int(entry_extent), _ptr(out), out.size,
+                               C.byref(nb), _ptr(stats))
+        if rc == UGVC_E_DATA:
+            rec, reason = C.c_int64(), C.c_int32()
+            lib.ugvc_hcr_error(self.h, lane, C.byref(rec), C.byref(reason))
+            err = UgvcDataError(rc, lib.ugvc_last_error(self.h).decode())
+            err.hcr_record, err.hcr_reason = int(rec.value), int(reason.value)
+            raise err
+        self._check(rc)
+        return {"bed": out[: nb.value].tobytes(), "n_lines": int(stats[0]), "skipped": int(stats[1]),
+                "exit_extent": int(stats[2]), "longest_segment": int(stats[3])}
+
+    def hcr_stage_ms(self, lane: int = 0) -> list[float]:
+        """ms of the last scan + emit on `lane`: H2D + inflate, index K1, decide + prefix max, emit kernels, D2H."""
+        ms = (C.c_float * 5)()
+        self._check(load_gvcf_hcr().ugvc_hcr_stage_ms(self.h, lane, C.cast(ms, C.c_void_p)))
+        return list(ms)
+
     def filter_bgzf_first_records(self, text_offsets, lane: int = 0) -> np.ndarray:
         """Index of the first record at or after each byte offset of the last filter_bgzf range's text."""
         off = np.ascontiguousarray(text_offsets, dtype=np.uint64)
@@ -842,6 +918,30 @@ def test_bsn(text: bytes, contigs: dict, params: BsnParams) -> dict:
         raise UgvcError(int(nb), "ugvc_test_bsn failed")
     return {"text": out[:nb].tobytes(), "line_start": out_ls, "rescued": rescued[:n].astype(bool), "hmer": hmer[:n],
             "end": end[:n], "n_rescued": int(nr.value)}
+
+
+def test_hcr(text: bytes, params: HcrParams, continues_contig: bool = False, entry_extent: int = -1, seg_bound: int = 0) -> dict:
+    """The gvcf_hcr kernels alone on whole lines with the given entry state (test hook ugvc_test_hcr, no context):
+    {"bed", "flags", "n_lines", "skipped", "exit_extent", "longest_segment"}, or {"error": (record, reason)} where the
+    reference raises."""
+    lib = load_gvcf_hcr()
+    buf = np.frombuffer(text, dtype=np.uint8)
+    nl = np.flatnonzero(buf == 10)  # noqa: PLR2004
+    ls = np.concatenate(([0], nl + 1)).astype(np.int64)
+    n = ls.size - 1
+    out = np.empty(buf.size + 48 * n + 16, np.uint8)
+    flags = np.empty(max(1, n), np.uint8)
+    stats = np.zeros(4, np.int64)
+    rec, reason = C.c_int64(), C.c_int32()
+    nb = lib.ugvc_test_hcr(_ptr(buf) if buf.size else None, buf.size, _ptr(ls), n, C.byref(params), int(bool(continues_contig)),
+                           int(entry_extent), int(seg_bound), _ptr(out), out.size, _ptr(flags), _ptr(stats), C.byref(rec),
+                           C.byref(reason))
+    if nb == UGVC_E_DATA:
+        return {"error": (int(rec.value), int(reason.value))}
+    if nb < 0:
+        raise UgvcError(int(nb), "ugvc_test_hcr failed")
+    return {"bed": out[:nb].tobytes(), "flags": flags[:n].copy(), "n_lines": int(stats[0]), "skipped": int(stats[1]),
+            "exit_extent": int(stats[2]), "longest_segment": int(stats[3])}
 
 
 def synth_header(n_custom: int) -> str:

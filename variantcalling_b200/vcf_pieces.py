@@ -1,4 +1,5 @@
-"""The device file path shared by the VCF-to-VCF tools (``low_af_ratio.py``, ``bridging_snvs.py``; DESIGN.md 4c, 4d).
+"""The device file path shared by the VCF tools (``low_af_ratio.py``, ``bridging_snvs.py``, ``gvcf_hcr.py``; DESIGN.md
+4c, 4d, 4e).
 
 The input (BGZF or plain text) is cut into pieces of whole lines of about ``piece_bytes`` of text, each piece is one
 device call, two pieces are in flight on two lanes, and the ``.tbi`` of the written records is built from the virtual
@@ -46,12 +47,13 @@ def inflate_block(raw: np.ndarray, coff: int, csize: int) -> bytes:
     return zlib.decompress(bytes(raw[coff + 12 + xlen: coff + csize - 8]), -15)
 
 
-def bgzf_cuts(path: str, raw: np.ndarray, coff, csz, ustart, data_begin: int, total: int, piece_bytes: int) -> list[int]:
+def bgzf_cuts(path: str, raw: np.ndarray, coff, csz, ustart, data_begin: int, total: int, piece_bytes: int,
+              index_cuts: bool = True) -> list[int]:
     """Uncompressed offsets where pieces begin (line starts), about piece_bytes apart: from the .tbi linear index when
-    there is one, else at the first line start of a block (that block inflated on the host)."""
+    there is one (and index_cuts), else at the first line start of a block (that block inflated on the host)."""
     cuts = [data_begin]
     cands: list[int] = []
-    if os.path.exists(path + ".tbi"):
+    if index_cuts and os.path.exists(path + ".tbi"):
         try:
             _, lin = bgzf_io.read_tbi(path + ".tbi", linear=True)
             voffs = np.unique(np.concatenate([v for v in lin.values()] or [np.zeros(0, np.uint64)]))
@@ -88,9 +90,10 @@ def text_cuts(text: np.ndarray, data_begin: int, piece_bytes: int) -> list[int]:
 
 class Input:
     """A VCF file cut into pieces of whole data lines: ``pieces[k] = (data, skip_head, take_bytes, span)`` as the device
-    calls take them, ``starts[k]`` the uncompressed offset of piece k's first line."""
+    calls take them, ``starts[k]`` the uncompressed offset of piece k's first line.  index_cuts=False cuts a BGZF file at
+    block line starts even when it has a ``.tbi``, so that pieces follow piece_bytes whatever the records' density."""
 
-    def __init__(self, path: str, data_begin: int, piece_bytes: int):
+    def __init__(self, path: str, data_begin: int, piece_bytes: int, index_cuts: bool = True):
         self.path = path
         raw = np.fromfile(path, dtype=np.uint8)
         self.raw = raw
@@ -99,7 +102,7 @@ class Input:
             self.coff, self.csz, usz = blocks(raw)
             self.ustart = np.concatenate(([0], np.cumsum(usz)))
             total = int(self.ustart[-1])
-            cuts = bgzf_cuts(path, raw, self.coff, self.csz, self.ustart[:-1], data_begin, total, piece_bytes)
+            cuts = bgzf_cuts(path, raw, self.coff, self.csz, self.ustart[:-1], data_begin, total, piece_bytes, index_cuts)
         else:
             cuts = text_cuts(raw, data_begin, piece_bytes)
         self.pieces, self.starts = [], []
@@ -126,15 +129,31 @@ class Input:
         out = []
         b = int(np.searchsorted(self.ustart, u0, side="right")) - 1
         while u0 < u1 and b < self.coff.size:
-            if self._cache[0] != b:
-                self._cache = (b, inflate_block(self.raw, int(self.coff[b]), int(self.csz[b])))
-            blk = self._cache[1]
+            cached = self._cache  # read once: the calls of the other lane's thread may replace it
+            if cached[0] != b:
+                cached = (b, inflate_block(self.raw, int(self.coff[b]), int(self.csz[b])))
+                self._cache = cached
+            blk = cached[1]
             lo = u0 - int(self.ustart[b])
             take = min(len(blk) - lo, u1 - u0)
             out.append(blk[lo: lo + take])
             u0 += take
             b += 1
         return b"".join(out)
+
+    def line_at(self, u0: int, r: int) -> str:
+        """Data line r of the piece that starts at uncompressed offset u0 (read back from the input)."""
+        at, chunk = u0, b""
+        for _ in range(r + 1):
+            at += len(chunk)
+            chunk = self.text(at, at + (1 << 16))
+            while b"\n" not in chunk:
+                more = self.text(at + len(chunk), at + len(chunk) + (1 << 16))
+                if not more:
+                    break
+                chunk += more
+            chunk = chunk[: chunk.find(b"\n") + 1] if b"\n" in chunk else chunk
+        return chunk.rstrip(b"\n").decode("latin-1")
 
 
 def run_on_lanes(ctx: lib.Context, n_pieces: int, call, thread_name: str):
