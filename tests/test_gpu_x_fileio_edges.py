@@ -275,3 +275,70 @@ def test_first_records_is_a_lower_bound_on_the_line_starts(gpu_ctx, job):
     bad = np.flatnonzero(res != want)
     assert bad.size == 0, [(int(offsets[i]), int(res[i]), int(want[i])) for i in bad[:8]]
     assert want[-1] == want[-2] == starts.size  # past the last line start: the record count
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# the range and capacity refusals of the file-path entry points
+# ---------------------------------------------------------------------------------------------------------------
+WHO = {"filter_bgzf_edits": "filter_bgzf", "filter_bgzf_split": "filter_bgzf_split", "afr_bgzf": "afr_bgzf",
+       "bsn_bgzf": "bsn_bgzf", "hcr_scan": "hcr_scan"}
+# out_capacity too small: the filter calls hand the range to the host writer, the tools refuse the argument
+OUT_TOO_SMALL = {"filter_bgzf_edits": lib.UGVC_E_FALLBACK, "filter_bgzf_split": lib.UGVC_E_FALLBACK,
+                 "afr_bgzf": lib.UGVC_E_ARG, "bsn_bgzf": lib.UGVC_E_ARG}
+
+
+def _call(entry: str, j: dict, comp: np.ndarray, skip_head: int, take_bytes: int, capacity_records: int,
+          out_capacity: int) -> tuple[int, int, str]:
+    """(rc, *out_n_records, ugvc_last_error) of one call of `entry` through ctypes, every output buffer sized for the
+    whole range and the capacities as given."""
+    ctx, n_max = j["ctx"], j["n_max"]
+    out = np.empty(len(j["text"]) * 2 + (1 << 20), np.uint8)
+    assert out_capacity <= out.size
+    blocks = np.empty(out.size // 65536 + 8, np.uint32)
+    ri, ls, ls2 = np.empty(n_max, lib.RECINFO_DTYPE), np.empty(n_max + 1, np.int64), np.empty(n_max + 1, np.int64)
+    u8, i64, i32, runs = np.empty(n_max, np.uint8), np.empty(n_max, np.int64), np.empty(n_max, np.int32), np.empty((n_max, 2), np.int64)
+    stats = np.zeros(8, np.int64)
+    nb, nblk, n, x = C.c_size_t(), C.c_size_t(), C.c_int64(-1), C.c_int64()
+    p = lib._ptr  # noqa: SLF001
+    src = (p(comp), comp.size, skip_head, take_bytes)
+    tail = (p(out), out_capacity, C.byref(nb), p(blocks), blocks.size, C.byref(nblk), p(ri), p(ls))
+    if entry in ("filter_bgzf_edits", "filter_bgzf_split"):
+        e, keep = lib._file_edits(True, False, j.get("blacklists"), None)  # noqa: F841, SLF001  (keep: alive for the call)
+        if entry == "filter_bgzf_edits":
+            rc = lib.load_library().ugvc_filter_bgzf_edits(ctx.h, 0, *src, 30.0, 0, C.byref(e), *tail, p(u8), capacity_records,
+                                                           C.byref(n))
+        else:
+            ma = j["ma"]
+            rc = lib.load_library().ugvc_filter_bgzf_split(ctx.h, j["index_ctx"].h, ma.h, 0, *src, p(ma.ref), ma.ref.size, 30.0,
+                                                           0, C.byref(e), *tail, p(u8), capacity_records, C.byref(n), p(stats))
+    elif entry == "afr_bgzf":
+        rc = lib.load_low_af_ratio().ugvc_afr_bgzf(ctx.h, 0, *src, 0, C.byref(j["params"]), *tail, p(i64), p(u8),
+                                                   capacity_records, C.byref(n), C.byref(x))
+    elif entry == "bsn_bgzf":
+        rc = lib.load_bridging_snvs().ugvc_bsn_bgzf(ctx.h, 0, *src, 0, C.byref(j["params"]), *tail, p(ls2), p(i64), p(u8), p(i32),
+                                                    capacity_records, C.byref(n), C.byref(x))
+    else:
+        rc = lib.load_gvcf_hcr().ugvc_hcr_scan(ctx.h, 0, *src, C.byref(j["params"]), capacity_records, C.byref(n), p(stats),
+                                               p(runs))
+    return rc, n.value, lib.load_library().ugvc_last_error(ctx.h).decode()
+
+
+@pytest.mark.parametrize("entry", list(WHO))
+def test_range_and_capacity_refusals(gpu_ctx, job, request, entry):
+    from tests.test_gpu_x_inflate_edges import ENTRIES
+
+    j = ENTRIES[entry][0](gpu_ctx, job[0], request)
+    text, who = j["text"], WHO[entry]
+    comp = np.frombuffer(bgzf_io.compress_bytes(text), dtype=np.uint8)
+    n_lines, big = text.count(b"\n"), len(text) * 2 + (1 << 20)
+    assert _call(entry, j, comp, 0, 0, j["n_max"], big)[:2] == (lib.UGVC_OK, n_lines)
+    assert _call(entry, j, comp, len(text) + 1, 0, j["n_max"], big)[::2] == (
+        lib.UGVC_E_ARG, f"{who}: skip_head beyond the inflated blocks")
+    assert _call(entry, j, comp, 0, len(text) + 1, j["n_max"], big)[::2] == (
+        lib.UGVC_E_ARG, f"{who}: the range is longer than the inflated blocks")
+    assert _call(entry, j, comp, 0, 0, n_lines - 1, big) == (
+        lib.UGVC_E_ARG, n_lines, f"{who}: output capacity smaller than the record count")
+    if entry in OUT_TOO_SMALL:
+        assert _call(entry, j, comp, 0, 0, j["n_max"], 16)[::2] == (
+            OUT_TOO_SMALL[entry], f"{who}: out_capacity smaller than the compressed output")
+    assert _call(entry, j, comp, 0, 0, j["n_max"], big)[:2] == (lib.UGVC_OK, n_lines)  # nothing sticks to the lane

@@ -216,23 +216,152 @@ def test_inflate_device_refuses_and_names_the_first_bad_block(ictx, ds):
     assert ictx.inflate_bgzf(good).tobytes() == text                   # nothing sticks to the context
 
 
-def test_filter_bgzf_refuses_and_names_the_first_bad_block(gpu_ctx, ds):
+def _split_vcf(full: str) -> tuple[str, bytes]:
+    """(header, data lines) of a whole VCF text."""
+    at = full.index("\n", full.index("#CHROM")) + 1
+    return full[:at], full[at:].encode()
+
+
+def _reserved(ctx, plan_blob: bytes, text: bytes, phreds: int = 0, grow: int = 1):
+    """The plan loaded and one lane reserved for `text`, or for `grow` times its bytes and lines (a split's scored pass)."""
+    ctx.load_plan(plan_blob)
+    if phreds:
+        ctx.enable_phreds(phreds)
+    ctx.reserve(grow * len(text) + (1 << 20), grow * text.count(b"\n") + 64, 1)
+
+
+def _bound(load):
+    """Bind a tool's entry points, or skip where the library lacks them (the host emulation of the filter path)."""
+    try:
+        load()
+    except AttributeError:
+        pytest.skip("the library lacks the tool's entry points: not part of the host emulation")
+
+
+# The device file-path entry points on one context each: set-up(gpu_ctx, ds, request) -> a job dict with the input
+# "text", the context "ctx", "n_max" (records the outputs hold) and what the entry needs besides.  run(job, bgzf bytes) ->
+# (record count, output bytes), or None where the entry hands the range back (the host emulation's stubs).
+def _setup_filter(ctx, ds, _request):
     _, tr, x = util.fit_transformer(ds)
     plan = MC.compile_plan(VcfHeader(ds["header_text"]), tr, util.fit_model("lr", x, ds["labels"]), ds["customs"])
-    gpu_ctx.load_plan(plan.blob)
-    gpu_ctx.reserve(len(ds["text"]) + (1 << 20), len(ds["lines"]) + 64, 1)
-    good, crc_bad, inc_bad, text = _bad_files(ds["text"])
-    n_max = len(ds["lines"]) + 64
-    res = gpu_ctx.filter_bgzf(np.frombuffer(good, np.uint8), 0, 0, 30.0, 0, n_max)
+    _reserved(ctx, plan.blob, ds["text"])
+    pos = np.unique([int(ln.split("\t", 2)[1]) for ln in ds["lines"][::7]]).astype(np.int64)
+    return {"text": ds["text"], "ctx": ctx, "n_max": len(ds["lines"]) + 64, "blacklists": [("BL_A;PASS", pos)]}
+
+
+def _setup_split(_ctx, _ds, request):
+    from tests.test_multiallelics_cpu import contig_text
+    from variantcalling_b200 import multiallelics as PM
+
+    mds, tr, model, _ = util.make_multiallelic_case(12, "lr")
+    hdr = VcfHeader(mds["header_text"])
+    text = contig_text(mds, "chrM1")
+    ctx, index_ctx = lib.Context(0), lib.Context(0)
+    ma = PM.DeviceSplitPlan(hdr, hdr.loader_columns(mds["customs"]), mds["ref"]["chrM1"])
+    for closer in (ctx.close, index_ctx.close, ma.close):
+        request.addfinalizer(closer)
+    _reserved(ctx, MC.compile_plan(hdr, tr, model, mds["customs"]).blob, text, phreds=2, grow=4)
+    _reserved(index_ctx, MC.compile_plan_no_model(hdr).blob, text)
+    return {"text": text, "ctx": ctx, "index_ctx": index_ctx, "ma": ma, "n_max": text.count(b"\n") + 64}
+
+
+def _setup_afr(ctx, _ds, _request):
+    from tests import low_af_ratio_data as LD
+
+    _bound(lib.load_low_af_ratio)
+    head, text = _split_vcf(LD.random_text(4000, 2, 21))
+    _reserved(ctx, MC.compile_plan_no_model(VcfHeader(head)).blob, text)
+    params = LD.params(head, af_ratio_threshold=5, af_ratio_threshold_h_indels=2, t_vaf_threshold=0.2)
+    return {"text": text, "ctx": ctx, "n_max": text.count(b"\n") + 64, "params": params}
+
+
+def _setup_bsn(ctx, _ds, request):
+    from tests import bridging_snvs_data as BD
+
+    _bound(lib.load_bridging_snvs)
+    g = BD.genome()
+    head, text = _split_vcf(BD.text(BD.random_records(g, 4000, 31)))
+    for name, seq in g.items():
+        ctx.bsn_add_contig(name, seq)
+    request.addfinalizer(ctx.bsn_clear_contigs)
+    _reserved(ctx, MC.compile_plan_no_model(VcfHeader(head)).blob, text)
+    return {"text": text, "ctx": ctx, "n_max": text.count(b"\n") + 64, "params": BD.params(head)}
+
+
+def _setup_hcr(ctx, _ds, _request):
+    from tests import gvcf_hcr_data as HD
+    from variantcalling_b200 import gvcf_hcr
+
+    _bound(lib.load_gvcf_hcr)
+    head, text = _split_vcf(HD.text(HD.random_records(4000, 7)))
+    _reserved(ctx, MC.compile_plan_no_model(VcfHeader(head)).blob, text)
+    return {"text": text, "ctx": ctx, "n_max": text.count(b"\n") + 64, "params": gvcf_hcr.hcr_params(VcfHeader(head))}
+
+
+def _run_filter(job, data):
+    res = job["ctx"].filter_bgzf(np.frombuffer(data, np.uint8), 0, 0, 30.0, 0, job["n_max"])
+    return None if res is None else (res["n_records"], res["bgzf"].tobytes())
+
+
+def _run_edits(job, data):
+    res = job["ctx"].filter_bgzf_edits(np.frombuffer(data, np.uint8), 0, 0, 30.0, 0, job["n_max"], blacklists=job["blacklists"])
+    return None if res is None else (res["n_records"], res["bgzf"].tobytes(), res["n_blacklisted"])
+
+
+def _run_split(job, data):
+    res = job["ma"].filter_bgzf(job["ctx"], job["index_ctx"], np.frombuffer(data, np.uint8), 0, 0, 30.0, 0, job["n_max"])
+    return None if res is None else (res["n_records"], res["bgzf"].tobytes())
+
+
+def _run_afr(job, data):
+    res = job["ctx"].afr_bgzf(np.frombuffer(data, np.uint8), 0, 0, False, job["params"], job["n_max"])
+    return res["n_records"], res["bgzf"].tobytes()
+
+
+def _run_bsn(job, data):
+    res = job["ctx"].bsn_bgzf(np.frombuffer(data, np.uint8), 0, 0, False, job["params"], job["n_max"])
+    return res["n_records"], res["bgzf"].tobytes()
+
+
+def _run_hcr(job, data):
+    ctx = job["ctx"]
+    res = ctx.hcr_scan(np.frombuffer(data, np.uint8), 0, 0, job["params"], job["n_max"])
+    return res["n_records"], ctx.hcr_emit(job["params"], False, -1, len(job["text"]) + 48 * res["n_records"] + 64)["bed"]
+
+
+ENTRIES = {"filter_bgzf": (_setup_filter, _run_filter), "filter_bgzf_edits": (_setup_filter, _run_edits),
+           "filter_bgzf_split": (_setup_split, _run_split), "afr_bgzf": (_setup_afr, _run_afr),
+           "bsn_bgzf": (_setup_bsn, _run_bsn), "hcr_scan": (_setup_hcr, _run_hcr)}
+
+
+def _refuses_and_names_the_first_bad_block(gpu_ctx, ds, request, entry):
+    setup, run = ENTRIES[entry]
+    job = setup(gpu_ctx, ds, request)
+    good, crc_bad, inc_bad, text = _bad_files(job["text"])
+    try:
+        res = run(job, good)
+    except lib.UgvcError as e:
+        if "host emulation" not in e.message:
+            raise
+        res = None
     if res is None:
-        pytest.skip("the device record writer is not part of the host emulation")
-    assert res["n_records"] == text.count(b"\n")
+        pytest.skip(f"the device file path of {entry} is not part of the host emulation")
+    assert res[0] == text.count(b"\n")
     for bad, where in ((crc_bad, r"block 1, code 9\)"), (inc_bad, r"block 2, code 3\)")):
         with pytest.raises(lib.UgvcError, match=where) as e:
-            gpu_ctx.filter_bgzf(np.frombuffer(bad, np.uint8), 0, 0, 30.0, 0, n_max)
+            run(job, bad)
         assert e.value.code == lib.UGVC_E_IO
-    again = gpu_ctx.filter_bgzf(np.frombuffer(good, np.uint8), 0, 0, 30.0, 0, n_max)
-    assert again["bgzf"].tobytes() == res["bgzf"].tobytes()
+    assert run(job, good) == res
+
+
+def test_filter_bgzf_refuses_and_names_the_first_bad_block(gpu_ctx, ds, request):
+    _refuses_and_names_the_first_bad_block(gpu_ctx, ds, request, "filter_bgzf")
+
+
+@pytest.mark.parametrize("entry", [e for e in ENTRIES if e != "filter_bgzf"])
+def test_file_path_entry_refuses_and_names_the_first_bad_block(gpu_ctx, ds, request, entry):
+    """The other device file-path entry points refuse the same blocks, and take a good input afterwards."""
+    _refuses_and_names_the_first_bad_block(gpu_ctx, ds, request, entry)
 
 
 def test_isize_zero_blocks_are_skipped_as_the_host_reader_skips_them(ictx):

@@ -280,6 +280,15 @@ static size_t align8(size_t x) { return (x + 7) & ~(size_t)7; }
 static int find_host_tag(const ugvc_ctx* ctx, const std::string& name);
 static std::string inf_err_message(int word);
 
+// After a synchronize: UGVC_E_IO naming the lowest failing block when the lane's last inflate failed.  The word is
+// cleared, so that the failure is reported once.
+static int take_inflate_error(ugvc_ctx* ctx, Lane& l) {
+    if (!l.h_inf_err || !*l.h_inf_err) return UGVC_OK;
+    const int code = *l.h_inf_err;
+    *l.h_inf_err = 0;
+    return fail(ctx, UGVC_E_IO, inf_err_message(code));
+}
+
 // Tables of the tile kernel (k1_tok): every INFO key it may meet -- the plan's tags declared in ##INFO
 // plus the keys seen in the data (`info_keys`, "KEY;KEY!;..." as for the key order; '!' marks a key that
 // came without a value) -- the usual FORMAT column, the kind bits of every slot, the fixed-column slots.
@@ -1031,12 +1040,9 @@ extern "C" int ugvc_collect_batch(ugvc_ctx* ctx, int lane, uint8_t* out_low_scor
     const int64_t n = *l.h_n;
     l.last_n = n;
     if (out_n_records) *out_n_records = n;
-    if (l.h_inf_err && *l.h_inf_err) {
-        const int code = *l.h_inf_err;
-        *l.h_inf_err = 0;
-        return fail(ctx, UGVC_E_IO, inf_err_message(code));
-    }
-    const int rc = decode_error(ctx, *l.h_err);
+    int rc = take_inflate_error(ctx, l);
+    if (rc) return rc;
+    rc = decode_error(ctx, *l.h_err);
     if (rc) return rc;
     if ((size_t)n > capacity_records) return fail(ctx, UGVC_E_ARG, "collect: output capacity smaller than the record count");
     const int K = ctx->plan.h.n_classes;
@@ -1329,11 +1335,8 @@ extern "C" int ugvc_bgzf_inflate_device(ugvc_ctx* ctx, const uint8_t* bgzf, size
     if (rc) return rc;
     if (out_n) *out_n = n_text;
     CU(cudaStreamSynchronize(l.stream));
-    if (l.h_inf_err && *l.h_inf_err) {
-        const int code = *l.h_inf_err;
-        *l.h_inf_err = 0;
-        return fail(ctx, UGVC_E_IO, inf_err_message(code));
-    }
+    rc = take_inflate_error(ctx, l);
+    if (rc) return rc;
     if (out_host) {
         if (n_text > capacity) return fail(ctx, UGVC_E_ARG, "bgzf_inflate_device: output capacity too small");
         CU(cudaMemcpy(out_host, l.d_text, n_text, cudaMemcpyDeviceToHost));
@@ -1484,7 +1487,7 @@ static int deflate_encoder() {
 
 // The encoder of the file path: f.d_out_text[0, n_text) (16 zero bytes after it: the encoder reads whole words) ->
 // n_blocks BGZF blocks (deflate), their sizes widened and scanned into offsets, the blocks packed back to back into
-// f.d_packed.  The sizes stay in f.d_bsize.
+// f.d_packed.  The sizes stay in f.d_bsize; their copy to f.h_bsize is enqueued (packed_bytes after a synchronize).
 static int encode_blocks(ugvc_ctx* ctx, Lane::FileBufs& f, size_t n_text, int n_blocks, int encoder, cudaStream_t st) {
     CU(cudaGetLastError());
     CU(fio_launch_deflate(f.d_out_text, n_text, ctx->d_def_tables, f.d_blocks, f.d_bsize, n_blocks, encoder, st));
@@ -1495,7 +1498,15 @@ static int encode_blocks(ugvc_ctx* ctx, Lane::FileBufs& f, size_t n_text, int n_
     CU(fio_scan_u64(f.d_scan_tmp, tmp, f.d_bwide, f.d_boff, n_blocks + 1, st));
     fio_launch_pack(f.d_blocks, f.d_bsize, f.d_bwide, f.d_boff, n_blocks, f.d_packed, ctx->sm_count, st);
     CU(cudaGetLastError());
+    f.h_bsize.resize((size_t)n_blocks + 1);
+    if (n_blocks) CU(cudaMemcpyAsync(f.h_bsize.data(), f.d_bsize, (size_t)n_blocks * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
     return UGVC_OK;
+}
+
+static size_t packed_bytes(const Lane::FileBufs& f, int n_blocks) {
+    size_t packed = 0;
+    for (int b = 0; b < n_blocks; ++b) packed += f.h_bsize[b];
+    return packed;
 }
 
 // The blacklists of a call to the device: positions (grown on demand), and one small block of position offsets, value
@@ -1597,6 +1608,110 @@ static int write_records(ugvc_ctx* ctx, Lane::FileBufs& f, const uint8_t* d_text
     return UGVC_OK;
 }
 
+// The record edits of a write_records call: flags, with_model, the phreds of n_classes classes (nullptr: no genotype
+// recalibration), the lane's blacklist mask, counter and INFO/END buffers, and the blacklists uploaded
+static int writer_edits(ugvc_ctx* ctx, Lane::FileBufs& f, const ugvc_file_edits& e, int flags, const double* phreds, int n_classes,
+                        cudaStream_t st, FioEdits& ed) {
+    ed = FioEdits{};
+    ed.with_model = e.with_model ? 1 : 0;
+    ed.flags = flags;
+    ed.phreds = phreds;
+    ed.n_classes = n_classes;
+    ed.bl_mask = f.d_bl_mask;
+    ed.n_blacklisted = f.d_n_bl;
+    ed.out_end = e.out_end ? f.d_end : nullptr;
+    return upload_blacklists(ctx, f, e, ed, st);
+}
+
+// The steps shared by the file-path calls, each entry point reading: its own checks, stage_range, index_pass, its own
+// kernels, encode_and_return.  `who` names the entry point in the error messages.
+//
+// The range's text on the device, its first byte 16-byte aligned, after event ev_start: whole BGZF blocks inflated and
+// [skip_head, skip_head + take_bytes) of them (take_bytes 0: to the end), or with is_text the caller's text uploaded,
+// TEXT_SLACK newlines after it.
+static int stage_range(ugvc_ctx* ctx, Lane& l, const std::string& who, const uint8_t* data, size_t n_bytes, uint32_t skip_head,
+                       uint64_t take_bytes, int is_text, cudaEvent_t ev_start, const uint8_t** d_text, size_t* n_text) {
+    cudaStream_t st = l.stream;
+    CU(cudaEventRecord(ev_start, st));
+    if (is_text) {
+        if (n_bytes > ctx->cap_bytes) return fail(ctx, UGVC_E_ARG, who + ": text larger than the reserved max_bytes");
+        *n_text = take_bytes ? (size_t)take_bytes : n_bytes;
+        if (*n_text > n_bytes) return fail(ctx, UGVC_E_ARG, who + ": take_bytes beyond the text");
+        CU(cudaMemcpyAsync(l.d_text, data, *n_text, cudaMemcpyHostToDevice, st));
+        CU(cudaMemsetAsync(l.d_text + *n_text, '\n', TEXT_SLACK, st));
+        *d_text = l.d_text;
+        return UGVC_OK;
+    }
+    const size_t shift = (16 - (skip_head & 15u)) & 15u;
+    size_t total = 0;
+    const int rc = stage_bgzf(ctx, l, data, n_bytes, inflate_decoder(), &total, shift);
+    if (rc) return rc;
+    if (skip_head > total) return fail(ctx, UGVC_E_ARG, who + ": skip_head beyond the inflated blocks");
+    *n_text = take_bytes ? (size_t)take_bytes : total - skip_head;
+    if (skip_head + *n_text > total) return fail(ctx, UGVC_E_ARG, who + ": the range is longer than the inflated blocks");
+    *d_text = l.d_text + shift + skip_head;
+    return UGVC_OK;
+}
+
+// The index pass on l's stream, between events ev[0] and ev[1]: K1..K3 of kctx's plan into its lane kl (ctx, l but for
+// ugvc_filter_bgzf_split, whose index pass runs in the model-less index context), the record count and error word to the
+// host; after a synchronize, l's inflate error (when the text was inflated), the data error, then *out_n and the
+// capacity check.  ctx takes kctx's message.
+static int index_pass(ugvc_ctx* ctx, Lane& l, ugvc_ctx* kctx, Lane& kl, const std::string& who, const uint8_t* d_text, size_t n_text,
+                      double threshold, bool inflated, size_t capacity_records, const cudaEvent_t* ev, int64_t* out_n) {
+    cudaStream_t st = l.stream;
+    CU(cudaEventRecord(ev[0], st));
+    int rc = enqueue_kernels(kctx, kl, d_text, n_text, threshold, kl.b.low_score, kl.b.probs, kl.b.qual, kl.b.recinfo, kl.b.line_start,
+                             kl.b.cap_records, kl.b.n_records, st);
+    if (rc) return fail(ctx, rc, kctx->err);
+    CU(cudaMemcpyAsync(kl.h_n, kl.b.n_records, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(kl.h_err, kl.d_err, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+    CU(cudaEventRecord(ev[1], st));
+    CU(cudaStreamSynchronize(st));
+    if (inflated) {
+        rc = take_inflate_error(ctx, l);
+        if (rc) return rc;
+    }
+    rc = decode_error(kctx, *kl.h_err);
+    if (rc) return fail(ctx, rc, kctx->err);
+    kl.last_n = *out_n = *kl.h_n;
+    if ((size_t)*out_n > capacity_records) return fail(ctx, UGVC_E_ARG, who + ": output capacity smaller than the record count");
+    return UGVC_OK;
+}
+
+// The output text at f.d_out_text[0, out_text), 16 zero bytes after it, deflated and packed between events ev[0] and
+// ev[1]; after a synchronize, the capacity check, then the copies of the blocks, their sizes, n records' recinfo (from
+// d_recinfo) and the output line starts to the host are enqueued; the caller adds its own, records its last event and
+// synchronizes.  writer_ran: write_records ran, and its fallback flag is read.  too_small: the code of an out_capacity
+// smaller than the blocks.  launches: the call's kernel launches besides the inflate and K1..K3.
+static int encode_and_return(ugvc_ctx* ctx, Lane& l, const std::string& who, size_t out_text, int64_t n, const ugvc_recinfo* d_recinfo,
+                             bool writer_ran, int too_small, int launches, const cudaEvent_t* ev, uint8_t* out_bgzf,
+                             size_t out_capacity, size_t* out_bytes, uint32_t* out_block_csize, size_t block_capacity,
+                             size_t* out_n_blocks, ugvc_recinfo* out_recinfo, int64_t* out_line_start) {
+    Lane::FileBufs& f = l.fb;
+    cudaStream_t st = l.stream;
+    CU(cudaEventRecord(ev[0], st));
+    const int n_blocks = (int)((out_text + DEF_CHUNK - 1) / DEF_CHUNK);
+    if ((size_t)n_blocks > f.cap_blocks || (out_block_csize && (size_t)n_blocks > block_capacity))
+        return fail(ctx, UGVC_E_ARG, who + ": more output blocks than room for them");
+    const int rc = encode_blocks(ctx, f, out_text, n_blocks, deflate_encoder(), st);
+    if (rc) return rc;
+    CU(cudaEventRecord(ev[1], st));
+    CU(cudaStreamSynchronize(st));
+    if (writer_ran && *f.h_fallback) return UGVC_E_FALLBACK;
+    const size_t packed = packed_bytes(f, n_blocks);
+    // the filter calls' callers sized out_bgzf for text that compresses, and can take their host writer instead
+    if (packed > out_capacity) return fail(ctx, too_small, who + ": out_capacity smaller than the compressed output");
+    ctx->launches += launches;
+    if (packed) CU(cudaMemcpyAsync(out_bgzf, f.d_packed, packed, cudaMemcpyDeviceToHost, st));
+    if (out_block_csize && n_blocks) memcpy(out_block_csize, f.h_bsize.data(), (size_t)n_blocks * sizeof(uint32_t));
+    if (out_recinfo && n) CU(cudaMemcpyAsync(out_recinfo, d_recinfo, (size_t)n * sizeof(ugvc_recinfo), cudaMemcpyDeviceToHost, st));
+    if (out_line_start) CU(cudaMemcpyAsync(out_line_start, f.d_out_ls, (size_t)(n + 1) * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    *out_bytes = packed;
+    if (out_n_blocks) *out_n_blocks = (size_t)n_blocks;
+    return UGVC_OK;
+}
+
 extern "C" int ugvc_filter_bgzf_edits(ugvc_ctx* ctx, int lane, const uint8_t* bgzf, size_t n_bytes, uint32_t skip_head,
                                       uint64_t take_bytes, double threshold, int flags, ugvc_file_edits* edits, uint8_t* out_bgzf,
                                       size_t out_capacity, size_t* out_bytes, uint32_t* out_block_csize, size_t block_capacity,
@@ -1622,72 +1737,24 @@ extern "C" int ugvc_filter_bgzf_edits(ugvc_ctx* ctx, int lane, const uint8_t* bg
     Lane::FileBufs& f = l.fb;
     cudaStream_t st = l.stream;
     (void)cudaGetLastError();  // nothing stale from this host thread's earlier calls
-    FioEdits ed{};
-    ed.with_model = e.with_model ? 1 : 0;
-    ed.flags = flags;
-    ed.phreds = e.recalibrate_genotype ? l.b.phreds : nullptr;
-    ed.n_classes = ctx->plan.h.n_classes;
-    ed.bl_mask = f.d_bl_mask;
-    ed.n_blacklisted = f.d_n_bl;
-    ed.out_end = e.out_end ? f.d_end : nullptr;
-    rc = upload_blacklists(ctx, f, e, ed, st);
+    FioEdits ed;
+    rc = writer_edits(ctx, f, e, flags, e.recalibrate_genotype ? l.b.phreds : nullptr, ctx->plan.h.n_classes, st, ed);
     if (rc) return rc;
-    CU(cudaEventRecord(f.ev[0], st));
-    // ---- compressed blocks -> text on the device, the range's first byte 16-byte aligned
-    const size_t shift = (16 - (skip_head & 15u)) & 15u;
-    size_t total = 0;
-    rc = stage_bgzf(ctx, l, bgzf, n_bytes, inflate_decoder(), &total, shift);
+    const uint8_t* d_text = nullptr;
+    size_t n_text = 0;
+    rc = stage_range(ctx, l, "filter_bgzf", bgzf, n_bytes, skip_head, take_bytes, 0, f.ev[0], &d_text, &n_text);
     if (rc) return rc;
-    if (skip_head > total) return fail(ctx, UGVC_E_ARG, "filter_bgzf: skip_head beyond the inflated blocks");
-    const size_t n_text = take_bytes ? (size_t)take_bytes : total - skip_head;
-    if (skip_head + n_text > total) return fail(ctx, UGVC_E_ARG, "filter_bgzf: the range is longer than the inflated blocks");
-    const uint8_t* d_text = l.d_text + shift + skip_head;
-    CU(cudaEventRecord(f.ev[1], st));
     // ---- K1..K3
-    rc = enqueue_kernels(ctx, l, d_text, n_text, threshold, l.b.low_score, l.b.probs, l.b.qual, l.b.recinfo, l.b.line_start,
-                         l.b.cap_records, l.b.n_records, st);
+    rc = index_pass(ctx, l, ctx, l, "filter_bgzf", d_text, n_text, threshold, true, capacity_records, f.ev + 1, out_n_records);
     if (rc) return rc;
-    CU(cudaMemcpyAsync(l.h_n, l.b.n_records, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
-    CU(cudaMemcpyAsync(l.h_err, l.d_err, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-    CU(cudaEventRecord(f.ev[2], st));
-    CU(cudaStreamSynchronize(st));
-    if (l.h_inf_err && *l.h_inf_err) {
-        const int code = *l.h_inf_err;
-        *l.h_inf_err = 0;
-        return fail(ctx, UGVC_E_IO, inf_err_message(code));
-    }
-    rc = decode_error(ctx, *l.h_err);
-    if (rc) return rc;
-    const int64_t n = *l.h_n;
-    l.last_n = n;
-    *out_n_records = n;
-    if ((size_t)n > capacity_records) return fail(ctx, UGVC_E_ARG, "filter_bgzf: output capacity smaller than the record count");
+    const int64_t n = *out_n_records;
     // ---- record writer
     size_t out_text = 0;
     rc = write_records(ctx, f, d_text, l.b.line_start, l.b.recinfo, l.b.low_score, l.b.qual, n, ed, st, &out_text);
     if (rc) return rc;
-    CU(cudaEventRecord(f.ev[3], st));
-    // ---- deflate, pack
-    const int n_blocks = (int)((out_text + DEF_CHUNK - 1) / DEF_CHUNK);
-    if ((size_t)n_blocks > f.cap_blocks || (out_block_csize && (size_t)n_blocks > block_capacity))
-        return fail(ctx, UGVC_E_ARG, "filter_bgzf: more output blocks than room for them");
-    rc = encode_blocks(ctx, f, out_text, n_blocks, deflate_encoder(), st);
+    rc = encode_and_return(ctx, l, "filter_bgzf", out_text, n, l.b.recinfo, true, UGVC_E_FALLBACK, 6, f.ev + 3, out_bgzf, out_capacity,
+                           out_bytes, out_block_csize, block_capacity, out_n_blocks, out_recinfo, out_line_start);
     if (rc) return rc;
-    f.h_bsize.resize((size_t)n_blocks + 1);
-    if (n_blocks) CU(cudaMemcpyAsync(f.h_bsize.data(), f.d_bsize, (size_t)n_blocks * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-    CU(cudaEventRecord(f.ev[4], st));
-    CU(cudaStreamSynchronize(st));
-    if (*f.h_fallback) return UGVC_E_FALLBACK;
-    size_t packed = 0;
-    for (int b = 0; b < n_blocks; ++b) packed += f.h_bsize[b];
-    if (packed > out_capacity)  // the caller sized out_bgzf for text that compresses; it can take its host writer instead
-        return fail(ctx, UGVC_E_FALLBACK, "filter_bgzf: out_capacity smaller than the compressed output");
-    ctx->launches += 6;
-    // ---- results to the host
-    if (packed) CU(cudaMemcpyAsync(out_bgzf, f.d_packed, packed, cudaMemcpyDeviceToHost, st));
-    if (out_block_csize && n_blocks) memcpy(out_block_csize, f.h_bsize.data(), (size_t)n_blocks * sizeof(uint32_t));
-    if (out_recinfo && n) CU(cudaMemcpyAsync(out_recinfo, l.b.recinfo, (size_t)n * sizeof(ugvc_recinfo), cudaMemcpyDeviceToHost, st));
-    if (out_line_start) CU(cudaMemcpyAsync(out_line_start, f.d_out_ls, (size_t)(n + 1) * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
     if (out_low_score && n) {
         if (e.with_model) CU(cudaMemcpyAsync(out_low_score, l.b.low_score, (size_t)n, cudaMemcpyDeviceToHost, st));
         else memset(out_low_score, 0, (size_t)n);  // no score: nothing is LOW_SCORE
@@ -1695,9 +1762,7 @@ extern "C" int ugvc_filter_bgzf_edits(ugvc_ctx* ctx, int lane, const uint8_t* bg
     if (e.out_end && n) CU(cudaMemcpyAsync(e.out_end, f.d_end, (size_t)n * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
     CU(cudaEventRecord(f.ev[5], st));
     CU(cudaStreamSynchronize(st));
-    *out_bytes = packed;
     edits->n_blacklisted = (int64_t)*f.h_n_bl;
-    if (out_n_blocks) *out_n_blocks = (size_t)n_blocks;
     for (int k = 0; k < 5; ++k) cudaEventElapsedTime(&f.ms[k], f.ev[k], f.ev[k + 1]);
     return UGVC_OK;
 }
@@ -1748,46 +1813,20 @@ extern "C" int ugvc_filter_bgzf_split(ugvc_ctx* ctx, ugvc_ctx* index_ctx, ugvc_m
         for (auto& ev : f.ev_split) CU(cudaEventCreate(&ev));
     cudaStream_t st = l.stream;
     (void)cudaGetLastError();
-    FioEdits ed{};
-    ed.with_model = 1;
-    ed.flags = flags;
-    ed.bl_mask = f.d_bl_mask;
-    ed.n_blacklisted = f.d_n_bl;
-    ed.out_end = e.out_end ? f.d_end : nullptr;
-    rc = upload_blacklists(ctx, f, e, ed, st);
+    FioEdits ed;  // the phreds and their width are the merge's, set below
+    rc = writer_edits(ctx, f, e, flags, nullptr, 0, st, ed);
     if (rc) return rc;
-    CU(cudaEventRecord(f.ev_split[0], st));
-    // ---- compressed blocks -> text on the device, the contig's first byte 16-byte aligned
-    const size_t shift = (16 - (skip_head & 15u)) & 15u;
-    size_t total = 0;
-    rc = stage_bgzf(ctx, l, bgzf, n_bytes, inflate_decoder(), &total, shift);
+    const uint8_t* d_text = nullptr;
+    size_t n_text = 0;
+    rc = stage_range(ctx, l, "filter_bgzf_split", bgzf, n_bytes, skip_head, take_bytes, 0, f.ev_split[0], &d_text, &n_text);
     if (rc) return rc;
-    if (skip_head > total) return fail(ctx, UGVC_E_ARG, "filter_bgzf_split: skip_head beyond the inflated blocks");
-    const size_t n_text = take_bytes ? (size_t)take_bytes : total - skip_head;
-    if (skip_head + n_text > total) return fail(ctx, UGVC_E_ARG, "filter_bgzf_split: the range is longer than the inflated blocks");
     if (n_text >= (1ull << 32) - 64u || n_text > index_ctx->cap_bytes)
         return fail(ctx, UGVC_E_FALLBACK, "filter_bgzf_split: the contig is beyond the device split's limits");
-    const uint8_t* d_text = l.d_text + shift + skip_head;
-    CU(cudaEventRecord(f.ev_split[1], st));
     // ---- index pass: K1 of the model-less plan into the index context's lane (the scored pass leaves them alone)
-    rc = enqueue_kernels(index_ctx, il, d_text, n_text, threshold, il.b.low_score, il.b.probs, il.b.qual, il.b.recinfo, il.b.line_start,
-                         il.b.cap_records, il.b.n_records, st);
-    if (rc) return fail(ctx, rc, index_ctx->err);
-    CU(cudaMemcpyAsync(il.h_n, il.b.n_records, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
-    CU(cudaMemcpyAsync(il.h_err, il.d_err, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-    CU(cudaEventRecord(f.ev_split[2], st));
-    CU(cudaStreamSynchronize(st));
-    if (l.h_inf_err && *l.h_inf_err) {
-        const int code = *l.h_inf_err;
-        *l.h_inf_err = 0;
-        return fail(ctx, UGVC_E_IO, inf_err_message(code));
-    }
-    rc = decode_error(index_ctx, *il.h_err);
-    if (rc) return fail(ctx, rc, index_ctx->err);
-    const int64_t n = *il.h_n;
-    il.last_n = n;
-    *out_n_records = n;
-    if ((size_t)n > capacity_records) return fail(ctx, UGVC_E_ARG, "filter_bgzf_split: output capacity smaller than the record count");
+    rc = index_pass(ctx, l, index_ctx, il, "filter_bgzf_split", d_text, n_text, threshold, true, capacity_records, f.ev_split + 1,
+                    out_n_records);
+    if (rc) return rc;
+    const int64_t n = *out_n_records;
     if ((size_t)n > l.b.cap_records) return fail(ctx, UGVC_E_FALLBACK, "filter_bgzf_split: more records than the reserved lane holds");
     // ---- split build (UGVC_E_DATA: the reference raises on this contig; out_split[7] = 1)
     rc = ma_build_on(ma, d_text, n_text, il.b.line_start, il.b.recinfo, n, ref_seq, ref_len, st, out_split);
@@ -1833,34 +1872,14 @@ extern "C" int ugvc_filter_bgzf_split(ugvc_ctx* ctx, ugvc_ctx* index_ctx, ugvc_m
     size_t out_text = 0;
     rc = write_records(ctx, f, d_text, il.b.line_start, il.b.recinfo, l.b.low_score, l.b.qual, n, ed, st, &out_text);
     if (rc) return rc;
-    CU(cudaEventRecord(f.ev_split[6], st));
-    // ---- deflate, pack
-    const int n_blocks = (int)((out_text + DEF_CHUNK - 1) / DEF_CHUNK);
-    if ((size_t)n_blocks > f.cap_blocks || (out_block_csize && (size_t)n_blocks > block_capacity))
-        return fail(ctx, UGVC_E_ARG, "filter_bgzf_split: more output blocks than room for them");
-    rc = encode_blocks(ctx, f, out_text, n_blocks, deflate_encoder(), st);
+    rc = encode_and_return(ctx, l, "filter_bgzf_split", out_text, n, il.b.recinfo, true, UGVC_E_FALLBACK, 7, f.ev_split + 6, out_bgzf,
+                           out_capacity, out_bytes, out_block_csize, block_capacity, out_n_blocks, out_recinfo, out_line_start);
     if (rc) return rc;
-    f.h_bsize.resize((size_t)n_blocks + 1);
-    if (n_blocks) CU(cudaMemcpyAsync(f.h_bsize.data(), f.d_bsize, (size_t)n_blocks * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-    CU(cudaEventRecord(f.ev_split[7], st));
-    CU(cudaStreamSynchronize(st));
-    if (*f.h_fallback) return UGVC_E_FALLBACK;
-    size_t packed = 0;
-    for (int b = 0; b < n_blocks; ++b) packed += f.h_bsize[b];
-    if (packed > out_capacity) return fail(ctx, UGVC_E_FALLBACK, "filter_bgzf_split: out_capacity smaller than the compressed output");
-    ctx->launches += 7;
-    // ---- results to the host
-    if (packed) CU(cudaMemcpyAsync(out_bgzf, f.d_packed, packed, cudaMemcpyDeviceToHost, st));
-    if (out_block_csize && n_blocks) memcpy(out_block_csize, f.h_bsize.data(), (size_t)n_blocks * sizeof(uint32_t));
-    if (out_recinfo && n) CU(cudaMemcpyAsync(out_recinfo, il.b.recinfo, (size_t)n * sizeof(ugvc_recinfo), cudaMemcpyDeviceToHost, st));
-    if (out_line_start) CU(cudaMemcpyAsync(out_line_start, f.d_out_ls, (size_t)(n + 1) * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
     if (out_low_score && n) CU(cudaMemcpyAsync(out_low_score, l.b.low_score, (size_t)n, cudaMemcpyDeviceToHost, st));
     if (e.out_end && n) CU(cudaMemcpyAsync(e.out_end, f.d_end, (size_t)n * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
     CU(cudaEventRecord(f.ev_split[8], st));
     CU(cudaStreamSynchronize(st));
-    *out_bytes = packed;
     edits->n_blacklisted = (int64_t)*f.h_n_bl;
-    if (out_n_blocks) *out_n_blocks = (size_t)n_blocks;
     for (int k = 0; k < 8; ++k) cudaEventElapsedTime(&f.ms_split[k], f.ev_split[k], f.ev_split[k + 1]);
     return UGVC_OK;
 }
@@ -1932,20 +1951,13 @@ extern "C" int64_t ugvc_test_write_records(ugvc_ctx* ctx, const uint8_t* text, s
     CU(cudaMemsetAsync(d_qual.p, 0, nn * sizeof(double), st));
     if (low_score && n) CU(cudaMemcpyAsync(d_low.p, low_score, (size_t)n, cudaMemcpyHostToDevice, st));
     if (qual && n) CU(cudaMemcpyAsync(d_qual.p, qual, (size_t)n * sizeof(double), cudaMemcpyHostToDevice, st));
-    FioEdits ed{};
-    ed.with_model = e.with_model ? 1 : 0;
-    ed.flags = flags;
-    ed.n_classes = n_classes;
     if (e.recalibrate_genotype) {
         const size_t np = nn * (size_t)(n_classes > 0 ? n_classes : 1);
         CU(cudaMalloc(&d_ph.p, np * sizeof(double)));
         if (n && n_classes > 0) CU(cudaMemcpyAsync(d_ph.p, phreds, (size_t)n * n_classes * sizeof(double), cudaMemcpyHostToDevice, st));
-        ed.phreds = static_cast<const double*>(d_ph.p);
     }
-    ed.bl_mask = f.d_bl_mask;
-    ed.n_blacklisted = f.d_n_bl;
-    ed.out_end = e.out_end ? f.d_end : nullptr;
-    rc = upload_blacklists(ctx, f, e, ed, st);
+    FioEdits ed;
+    rc = writer_edits(ctx, f, e, flags, static_cast<const double*>(d_ph.p), n_classes, st, ed);
     if (rc) return rc;
     size_t out_text = 0;
     rc = write_records(ctx, f, l.d_text, l.b.line_start, l.b.recinfo, static_cast<const uint8_t*>(d_low.p),
@@ -2007,11 +2019,8 @@ extern "C" int ugvc_test_device_deflate(ugvc_ctx* ctx, const uint8_t* data, size
     CU(cudaMemsetAsync(f.d_out_text + n, 0, 16, st));
     rc = encode_blocks(ctx, f, n, n_blocks, encoder, st);
     if (rc) return rc;
-    f.h_bsize.resize((size_t)n_blocks + 1);
-    if (n_blocks) CU(cudaMemcpyAsync(f.h_bsize.data(), f.d_bsize, (size_t)n_blocks * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
-    size_t packed = 0;
-    for (int b = 0; b < n_blocks; ++b) packed += f.h_bsize[b];
+    const size_t packed = packed_bytes(f, n_blocks);
     if (packed > capacity || (packed && !out)) return fail(ctx, UGVC_E_ARG, "test_device_deflate: capacity smaller than the compressed output");
     if (packed) CU(cudaMemcpyAsync(out, f.d_packed, packed, cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
@@ -2021,15 +2030,13 @@ extern "C" int ugvc_test_device_deflate(ugvc_ctx* ctx, const uint8_t* data, size
     return UGVC_OK;
 }
 
-// The first half of a VCF-to-VCF tool call (ugvc_afr_bgzf, ugvc_bsn_bgzf): the scan scratch, the range's text on the
-// device (inflated, or uploaded plain) and the index pass (line starts, POS, len(REF)); events ev[0..2].
+// The front of a VCF-to-VCF tool call (ugvc_afr_bgzf, ugvc_bsn_bgzf, ugvc_hcr_scan): the scan scratch, the range's text
+// on the device (inflated, or uploaded plain) and the index pass (line starts, POS, len(REF)); events ev[0..2].
 static int tool_front(ugvc_ctx* ctx, Lane& l, const char* who, const uint8_t* data, size_t n_bytes, uint32_t skip_head,
-                      uint64_t take_bytes, int is_text, size_t capacity_records, const uint8_t** d_text_out, int64_t* n_out) {
-    const std::string w(who);
+                      uint64_t take_bytes, int is_text, size_t capacity_records, const uint8_t** d_text, int64_t* n_out) {
     int rc = file_bufs(ctx, l);
     if (rc) return rc;
     Lane::FileBufs& f = l.fb;
-    cudaStream_t st = l.stream;
     (void)cudaGetLastError();
     if (!f.d_afr_tot) {
         CU(cudaMalloc(&f.d_afr_tot, 3 * sizeof(int64_t)));
@@ -2043,84 +2050,20 @@ static int tool_front(ugvc_ctx* ctx, Lane& l, const char* who, const uint8_t* da
         CU(cudaMalloc(&f.d_afr_agg, need_agg * sizeof(int64_t)));
         f.cap_afr_agg = need_agg;
     }
-    CU(cudaEventRecord(f.ev[0], st));
-    // ---- the range's text on the device, its first byte 16-byte aligned
-    const uint8_t* d_text = nullptr;
     size_t n_text = 0;
-    if (is_text) {
-        if (n_bytes > ctx->cap_bytes) return fail(ctx, UGVC_E_ARG, w + ": text larger than the reserved max_bytes");
-        n_text = take_bytes ? (size_t)take_bytes : n_bytes;
-        if (n_text > n_bytes) return fail(ctx, UGVC_E_ARG, w + ": take_bytes beyond the text");
-        CU(cudaMemcpyAsync(l.d_text, data, n_text, cudaMemcpyHostToDevice, st));
-        CU(cudaMemsetAsync(l.d_text + n_text, '\n', TEXT_SLACK, st));
-        d_text = l.d_text;
-    } else {
-        const size_t shift = (16 - (skip_head & 15u)) & 15u;
-        size_t total = 0;
-        rc = stage_bgzf(ctx, l, data, n_bytes, inflate_decoder(), &total, shift);
-        if (rc) return rc;
-        if (skip_head > total) return fail(ctx, UGVC_E_ARG, w + ": skip_head beyond the inflated blocks");
-        n_text = take_bytes ? (size_t)take_bytes : total - skip_head;
-        if (skip_head + n_text > total) return fail(ctx, UGVC_E_ARG, w + ": the range is longer than the inflated blocks");
-        d_text = l.d_text + shift + skip_head;
-    }
-    CU(cudaEventRecord(f.ev[1], st));
-    // ---- index pass: line starts, POS, len(REF)
-    rc = enqueue_kernels(ctx, l, d_text, n_text, 0.0, l.b.low_score, l.b.probs, l.b.qual, l.b.recinfo, l.b.line_start,
-                         l.b.cap_records, l.b.n_records, st);
+    rc = stage_range(ctx, l, who, data, n_bytes, skip_head, take_bytes, is_text, f.ev[0], d_text, &n_text);
     if (rc) return rc;
-    CU(cudaMemcpyAsync(l.h_n, l.b.n_records, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
-    CU(cudaMemcpyAsync(l.h_err, l.d_err, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-    CU(cudaEventRecord(f.ev[2], st));
-    CU(cudaStreamSynchronize(st));
-    if (!is_text && l.h_inf_err && *l.h_inf_err) {
-        const int code = *l.h_inf_err;
-        *l.h_inf_err = 0;
-        return fail(ctx, UGVC_E_IO, inf_err_message(code));
-    }
-    rc = decode_error(ctx, *l.h_err);
-    if (rc) return rc;
-    const int64_t n = *l.h_n;
-    l.last_n = n;
-    *n_out = n;
-    if ((size_t)n > capacity_records) return fail(ctx, UGVC_E_ARG, w + ": output capacity smaller than the record count");
-    *d_text_out = d_text;
-    return UGVC_OK;
+    return index_pass(ctx, l, ctx, l, who, *d_text, n_text, 0.0, !is_text, capacity_records, f.ev + 1, n_out);
 }
 
-// The second half, after the tool's copy kernel has written out_text bytes at fb.d_out_text: deflate and pack (events
-// ev[3..4]), then the D2H of the blocks, recinfo and the output line starts is enqueued; the caller adds its own copies,
-// records ev[5] and synchronizes.
-static int tool_back(ugvc_ctx* ctx, Lane& l, const char* who, size_t out_text, int64_t n, uint8_t* out_bgzf, size_t out_capacity,
-                     size_t* out_bytes, uint32_t* out_block_csize, size_t block_capacity, size_t* out_n_blocks,
-                     ugvc_recinfo* out_recinfo, int64_t* out_line_start) {
-    const std::string w(who);
-    Lane::FileBufs& f = l.fb;
-    cudaStream_t st = l.stream;
-    CU(cudaMemsetAsync(f.d_out_text + out_text, 0, 16, st));  // the encoder reads whole words
-    CU(cudaEventRecord(f.ev[3], st));
-    // ---- deflate, pack
-    const int n_blocks = (int)((out_text + DEF_CHUNK - 1) / DEF_CHUNK);
-    if ((size_t)n_blocks > f.cap_blocks || (out_block_csize && (size_t)n_blocks > block_capacity))
-        return fail(ctx, UGVC_E_ARG, w + ": more output blocks than room for them");
-    int rc = encode_blocks(ctx, f, out_text, n_blocks, deflate_encoder(), st);
-    if (rc) return rc;
-    f.h_bsize.resize((size_t)n_blocks + 1);
-    if (n_blocks) CU(cudaMemcpyAsync(f.h_bsize.data(), f.d_bsize, (size_t)n_blocks * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-    CU(cudaEventRecord(f.ev[4], st));
-    CU(cudaStreamSynchronize(st));
-    size_t packed = 0;
-    for (int b = 0; b < n_blocks; ++b) packed += f.h_bsize[b];
-    if (packed > out_capacity) return fail(ctx, UGVC_E_ARG, w + ": out_capacity smaller than the compressed output");
-    ctx->launches += 9;
-    // ---- results to the host
-    if (packed) CU(cudaMemcpyAsync(out_bgzf, f.d_packed, packed, cudaMemcpyDeviceToHost, st));
-    if (out_block_csize && n_blocks) memcpy(out_block_csize, f.h_bsize.data(), (size_t)n_blocks * sizeof(uint32_t));
-    if (out_recinfo && n) CU(cudaMemcpyAsync(out_recinfo, l.b.recinfo, (size_t)n * sizeof(ugvc_recinfo), cudaMemcpyDeviceToHost, st));
-    if (out_line_start) CU(cudaMemcpyAsync(out_line_start, f.d_out_ls, (size_t)(n + 1) * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
-    *out_bytes = packed;
-    if (out_n_blocks) *out_n_blocks = (size_t)n_blocks;
-    return UGVC_OK;
+// A tool kernel's error word: AFR_NO_ERROR, or the first record the reference raises at (err >> 4) and the reason
+// (err & 0xF), kept in the tool's own fields for its ugvc_*_error query
+static int tool_data_error(ugvc_ctx* ctx, const std::string& who, unsigned long long err, int64_t& record, int32_t& reason) {
+    if (err == AFR_NO_ERROR) return UGVC_OK;
+    record = (int64_t)(err >> 4);
+    reason = (int32_t)(err & 0xF);
+    return fail(ctx, UGVC_E_DATA, who + ": the reference raises at record " + std::to_string(record) + " (reason " +
+                                      std::to_string(reason) + ")");
 }
 
 // filter_low_af_ratio_to_background, file to file: inflate (or upload) -> index K1 -> afr decide / scan / copy -> deflate
@@ -2156,20 +2099,16 @@ extern "C" int ugvc_afr_bgzf(ugvc_ctx* ctx, int lane, const uint8_t* data, size_
     if (n == 0) CU(cudaMemsetAsync(f.d_afr_tot, 0, 2 * sizeof(int64_t), st));
     CU(cudaMemcpyAsync(f.h_afr_tot, f.d_afr_tot, 3 * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
-    const unsigned long long err = (unsigned long long)f.h_afr_tot[2];
-    if (err != AFR_NO_ERROR) {
-        f.afr_err_record = (int64_t)(err >> 4);
-        f.afr_err_reason = (int32_t)(err & 0xF);
-        return fail(ctx, UGVC_E_DATA, "afr_bgzf: the reference raises at record " + std::to_string(f.afr_err_record) + " (reason " +
-                                          std::to_string(f.afr_err_reason) + ")");
-    }
+    rc = tool_data_error(ctx, "afr_bgzf", (unsigned long long)f.h_afr_tot[2], f.afr_err_record, f.afr_err_reason);
+    if (rc) return rc;
     const size_t out_text = (size_t)f.h_afr_tot[0];
     const int64_t n_failed = f.h_afr_tot[1];
     if (out_text > f.cap_out) return fail(ctx, UGVC_E_ARG, "afr_bgzf: the written text exceeds the writer's buffer");
     if (n == 0) CU(cudaMemsetAsync(f.d_out_ls, 0, sizeof(int64_t), st));
     afr_launch_copy(d_text, l.b.line_start, n, P, f.d_score, f.d_out_ls, f.d_out_text, ctx->sm_count, st);
-    rc = tool_back(ctx, l, "afr_bgzf", out_text, n, out_bgzf, out_capacity, out_bytes, out_block_csize, block_capacity, out_n_blocks,
-                   out_recinfo, out_line_start);
+    CU(cudaMemsetAsync(f.d_out_text + out_text, 0, 16, st));  // the encoder reads whole words
+    rc = encode_and_return(ctx, l, "afr_bgzf", out_text, n, l.b.recinfo, false, UGVC_E_ARG, 9, f.ev + 3, out_bgzf, out_capacity, out_bytes,
+                           out_block_csize, block_capacity, out_n_blocks, out_recinfo, out_line_start);
     if (rc) return rc;
     if (out_end && n) CU(cudaMemcpyAsync(out_end, f.d_end, (size_t)n * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
     if (out_flags && n) CU(cudaMemcpyAsync(out_flags, f.d_score, (size_t)n, cudaMemcpyDeviceToHost, st));
@@ -2288,20 +2227,16 @@ extern "C" int ugvc_bsn_bgzf(ugvc_ctx* ctx, int lane, const uint8_t* data, size_
     if (n == 0) CU(cudaMemsetAsync(f.d_afr_tot, 0, 2 * sizeof(int64_t), st));
     CU(cudaMemcpyAsync(f.h_afr_tot, f.d_afr_tot, 3 * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
-    const unsigned long long err = (unsigned long long)f.h_afr_tot[2];
-    if (err != AFR_NO_ERROR) {
-        f.bsn_err_record = (int64_t)(err >> 4);
-        f.bsn_err_reason = (int32_t)(err & 0xF);
-        return fail(ctx, UGVC_E_DATA, "bsn_bgzf: the reference raises at record " + std::to_string(f.bsn_err_record) + " (reason " +
-                                          std::to_string(f.bsn_err_reason) + ")");
-    }
+    rc = tool_data_error(ctx, "bsn_bgzf", (unsigned long long)f.h_afr_tot[2], f.bsn_err_record, f.bsn_err_reason);
+    if (rc) return rc;
     const size_t out_text = (size_t)f.h_afr_tot[0];
     const int64_t n_rescued = f.h_afr_tot[1];
     if (out_text > f.cap_out) return fail(ctx, UGVC_E_ARG, "bsn_bgzf: the written text exceeds the writer's buffer");
     if (n == 0) CU(cudaMemsetAsync(f.d_out_ls, 0, sizeof(int64_t), st));
     bsn_launch_copy(d_text, l.b.line_start, n, P, f.d_score, f.d_out_ls, f.d_out_text, ctx->sm_count, st);
-    rc = tool_back(ctx, l, "bsn_bgzf", out_text, n, out_bgzf, out_capacity, out_bytes, out_block_csize, block_capacity, out_n_blocks,
-                   out_recinfo, out_line_start);
+    CU(cudaMemsetAsync(f.d_out_text + out_text, 0, 16, st));  // the encoder reads whole words
+    rc = encode_and_return(ctx, l, "bsn_bgzf", out_text, n, l.b.recinfo, false, UGVC_E_ARG, 9, f.ev + 3, out_bgzf, out_capacity, out_bytes,
+                           out_block_csize, block_capacity, out_n_blocks, out_recinfo, out_line_start);
     if (rc) return rc;
     if (out_src_line_start) CU(cudaMemcpyAsync(out_src_line_start, l.b.line_start, (size_t)(n + 1) * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
     if (out_end && n) CU(cudaMemcpyAsync(out_end, f.d_end, (size_t)n * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
@@ -2390,12 +2325,8 @@ extern "C" int ugvc_hcr_emit(ugvc_ctx* ctx, int lane, const ugvc_hcr_params* par
     out_stats[1] = r.skipped;
     out_stats[2] = r.exit_extent;
     out_stats[3] = r.longest;
-    if ((unsigned long long)r.err != AFR_NO_ERROR) {
-        f.hcr_err_record = (int64_t)((unsigned long long)r.err >> 4);
-        f.hcr_err_reason = (int32_t)((unsigned long long)r.err & 0xF);
-        return fail(ctx, UGVC_E_DATA, "hcr_emit: the reference raises at record " + std::to_string(f.hcr_err_record) + " (reason " +
-                                          std::to_string(f.hcr_err_reason) + ")");
-    }
+    const int rc = tool_data_error(ctx, "hcr_emit", (unsigned long long)r.err, f.hcr_err_record, f.hcr_err_reason);
+    if (rc) return rc;
     if ((size_t)r.bytes > out_capacity || (r.bytes && !out_bed)) return fail(ctx, UGVC_E_ARG, "hcr_emit: out_capacity smaller than the BED text");
     if (r.bytes) CU(cudaMemcpyAsync(out_bed, f.d_out_text, (size_t)r.bytes, cudaMemcpyDeviceToHost, st));
     CU(cudaEventRecord(f.ev_hcr[3], st));

@@ -208,21 +208,23 @@ SIGNATURES = {
                                   _vp, _vp, _i64p, C.POINTER(C.c_int32)]),
 }
 
-# the concordance-frame annotation entry points are bound on first use (load_annotation), so that a build of the
-# library without them, such as the host emulation of the filter path, still loads
-_BOUND_ON_USE = frozenset(n for n in SIGNATURES if n.startswith("ugvc_conc_annot"))
-# so are those of filter_low_af_ratio_to_background (load_low_af_ratio)
-_AFR_BOUND_ON_USE = frozenset(n for n in SIGNATURES if n.startswith(("ugvc_afr_", "ugvc_test_afr")))
-# and those of calibrate_bridging_snvs (load_bridging_snvs)
-_BSN_BOUND_ON_USE = frozenset(n for n in SIGNATURES if n.startswith(("ugvc_bsn_", "ugvc_test_bsn")))
-# and those of gvcf_hcr (load_gvcf_hcr)
-_HCR_BOUND_ON_USE = frozenset(n for n in SIGNATURES if n.startswith(("ugvc_hcr_", "ugvc_test_hcr")))
+# the entry points of the concordance-frame annotation and of each VCF-to-VCF tool, by name prefix, are bound on first use
+# (load_annotation, load_low_af_ratio, ...), so that a build of the library without them, such as the host emulation of
+# the filter path, still loads
+_ANNOTATION, _AFR = ("ugvc_conc_annot",), ("ugvc_afr_", "ugvc_test_afr")
+_BSN, _HCR = ("ugvc_bsn_", "ugvc_test_bsn"), ("ugvc_hcr_", "ugvc_test_hcr")
+_BOUND_ON_USE = frozenset(n for n in SIGNATURES if n.startswith(_ANNOTATION + _AFR + _BSN + _HCR))
+_groups_bound: set[tuple] = set()
 
 _lib = None
-_annotation_bound = False
-_afr_bound = False
-_bsn_bound = False
-_hcr_bound = False
+
+
+def _bind(lib: C.CDLL, names):
+    for name in names:
+        res, args = SIGNATURES[name]
+        fn = getattr(lib, name)
+        fn.restype = res
+        fn.argtypes = args
 
 
 def load_library() -> C.CDLL:
@@ -234,70 +236,38 @@ def load_library() -> C.CDLL:
                 f"{LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
                 f"(make -C variantcalling_b200/csrc).  There is no CPU fallback for the hot path.")
         lib = C.CDLL(LIB_PATH)
-        for name, (res, args) in SIGNATURES.items():
-            if name in _BOUND_ON_USE or name in _AFR_BOUND_ON_USE or name in _BSN_BOUND_ON_USE or name in _HCR_BOUND_ON_USE:
-                continue
-            fn = getattr(lib, name)
-            fn.restype = res
-            fn.argtypes = args
+        _bind(lib, [name for name in SIGNATURES if name not in _BOUND_ON_USE])
         _lib = lib
     return _lib
 
 
+def _load_group(prefix: tuple) -> C.CDLL:
+    """load_library() with the entry points named `prefix` bound.  Raises if the library lacks them."""
+    lib = load_library()
+    if prefix not in _groups_bound:
+        _bind(lib, sorted(n for n in SIGNATURES if n.startswith(prefix)))
+        _groups_bound.add(prefix)
+    return lib
+
+
 def load_annotation() -> C.CDLL:
     """load_library() with the annotation entry points bound.  Raises if the library lacks them."""
-    global _annotation_bound  # noqa: PLW0603
-    lib = load_library()
-    if not _annotation_bound:
-        for name in sorted(_BOUND_ON_USE):
-            res, args = SIGNATURES[name]
-            fn = getattr(lib, name)
-            fn.restype = res
-            fn.argtypes = args
-        _annotation_bound = True
-    return lib
+    return _load_group(_ANNOTATION)
 
 
 def load_low_af_ratio() -> C.CDLL:
     """load_library() with the filter_low_af_ratio_to_background entry points bound.  Raises if the library lacks them."""
-    global _afr_bound  # noqa: PLW0603
-    lib = load_library()
-    if not _afr_bound:
-        for name in sorted(_AFR_BOUND_ON_USE):
-            res, args = SIGNATURES[name]
-            fn = getattr(lib, name)
-            fn.restype = res
-            fn.argtypes = args
-        _afr_bound = True
-    return lib
+    return _load_group(_AFR)
 
 
 def load_bridging_snvs() -> C.CDLL:
     """load_library() with the calibrate_bridging_snvs entry points bound.  Raises if the library lacks them."""
-    global _bsn_bound  # noqa: PLW0603
-    lib = load_library()
-    if not _bsn_bound:
-        for name in sorted(_BSN_BOUND_ON_USE):
-            res, args = SIGNATURES[name]
-            fn = getattr(lib, name)
-            fn.restype = res
-            fn.argtypes = args
-        _bsn_bound = True
-    return lib
+    return _load_group(_BSN)
 
 
 def load_gvcf_hcr() -> C.CDLL:
     """load_library() with the gvcf_hcr entry points bound.  Raises if the library lacks them."""
-    global _hcr_bound  # noqa: PLW0603
-    lib = load_library()
-    if not _hcr_bound:
-        for name in sorted(_HCR_BOUND_ON_USE):
-            res, args = SIGNATURES[name]
-            fn = getattr(lib, name)
-            fn.restype = res
-            fn.argtypes = args
-        _hcr_bound = True
-    return lib
+    return _load_group(_HCR)
 
 
 def _ptr(a):
@@ -376,6 +346,18 @@ class Context:
         if rc == UGVC_E_DATA:
             raise UgvcDataError(rc, msg)
         raise UgvcError(rc, msg)
+
+    def _check_tool(self, rc: int, query, tool: str, lane: int):
+        """_check for a VCF-to-VCF tool call: UGVC_E_DATA raises UgvcDataError with .<tool>_record / .<tool>_reason, the
+        record the reference raises at and why, from the tool's error query (`query`, e.g. ugvc_afr_error)."""
+        if rc == UGVC_E_DATA:
+            rec, reason = C.c_int64(), C.c_int32()
+            query(self.h, lane, C.byref(rec), C.byref(reason))
+            err = UgvcDataError(rc, self.lib.ugvc_last_error(self.h).decode())
+            setattr(err, f"{tool}_record", int(rec.value))
+            setattr(err, f"{tool}_reason", int(reason.value))
+            raise err
+        self._check(rc)
 
     def close(self):
         if self.h:
@@ -629,13 +611,7 @@ class Context:
         rc = lib.ugvc_afr_bgzf(self.h, lane, _ptr(src), src.size, skip_head, take_bytes, int(bool(is_text)), C.byref(params),
                                _ptr(out), out.size, C.byref(nb), _ptr(blocks), blocks.size, C.byref(nblk), _ptr(ri), _ptr(ls),
                                _ptr(end), _ptr(flags), max_records, C.byref(n), C.byref(nf))
-        if rc == UGVC_E_DATA:
-            rec, reason = C.c_int64(), C.c_int32()
-            lib.ugvc_afr_error(self.h, lane, C.byref(rec), C.byref(reason))
-            err = UgvcDataError(rc, lib.ugvc_last_error(self.h).decode())
-            err.afr_record, err.afr_reason = int(rec.value), int(reason.value)
-            raise err
-        self._check(rc)
+        self._check_tool(rc, lib.ugvc_afr_error, "afr", lane)
         k = n.value
         return {"n_records": k, "n_filtered": int(nf.value), "bgzf": out[: nb.value], "block_csize": blocks[: nblk.value],
                 "recinfo": ri[:k], "line_start": ls[: k + 1], "end": end[:k], "flags": flags[:k]}
@@ -674,13 +650,7 @@ class Context:
         rc = lib.ugvc_bsn_bgzf(self.h, lane, _ptr(src), src.size, skip_head, take_bytes, int(bool(is_text)), C.byref(params),
                                _ptr(out), out.size, C.byref(nb), _ptr(blocks), blocks.size, C.byref(nblk), _ptr(ri), _ptr(ls),
                                _ptr(src_ls), _ptr(end), _ptr(flags), _ptr(hmer), max_records, C.byref(n), C.byref(nr))
-        if rc == UGVC_E_DATA:
-            rec, reason = C.c_int64(), C.c_int32()
-            lib.ugvc_bsn_error(self.h, lane, C.byref(rec), C.byref(reason))
-            err = UgvcDataError(rc, lib.ugvc_last_error(self.h).decode())
-            err.bsn_record, err.bsn_reason = int(rec.value), int(reason.value)
-            raise err
-        self._check(rc)
+        self._check_tool(rc, lib.ugvc_bsn_error, "bsn", lane)
         k = n.value
         return {"n_records": k, "n_rescued": int(nr.value), "bgzf": out[: nb.value], "block_csize": blocks[: nblk.value],
                 "recinfo": ri[:k], "line_start": ls[: k + 1], "src_line_start": src_ls[: k + 1], "end": end[:k],
@@ -718,13 +688,7 @@ class Context:
         nb = C.c_size_t()
         rc = lib.ugvc_hcr_emit(self.h, lane, C.byref(params), int(bool(continues_contig)), int(entry_extent), _ptr(out), out.size,
                                C.byref(nb), _ptr(stats))
-        if rc == UGVC_E_DATA:
-            rec, reason = C.c_int64(), C.c_int32()
-            lib.ugvc_hcr_error(self.h, lane, C.byref(rec), C.byref(reason))
-            err = UgvcDataError(rc, lib.ugvc_last_error(self.h).decode())
-            err.hcr_record, err.hcr_reason = int(rec.value), int(reason.value)
-            raise err
-        self._check(rc)
+        self._check_tool(rc, lib.ugvc_hcr_error, "hcr", lane)
         return {"bed": out[: nb.value].tobytes(), "n_lines": int(stats[0]), "skipped": int(stats[1]),
                 "exit_extent": int(stats[2]), "longest_segment": int(stats[3])}
 
@@ -866,14 +830,18 @@ class Context:
         return list(arr), n.value
 
 
+def _lines(text: bytes) -> tuple[np.ndarray, np.ndarray, int]:
+    """(bytes, line starts with the end after them, line count) of whole lines, for the kernel test hooks."""
+    buf = np.frombuffer(text, dtype=np.uint8)
+    ls = np.concatenate(([0], np.flatnonzero(buf == 10) + 1)).astype(np.int64)  # noqa: PLR2004
+    return buf, ls, ls.size - 1
+
+
 def test_afr(text: bytes, params: AfrParams) -> dict:
     """The filter_low_af_ratio_to_background kernels alone on whole lines (test hook ugvc_test_afr, no context):
     {"text", "line_start", "failed", "end", "n_filtered"}, or {"error": (record, reason)} where the reference raises."""
     lib = load_low_af_ratio()
-    buf = np.frombuffer(text, dtype=np.uint8)
-    nl = np.flatnonzero(buf == 10)  # noqa: PLR2004
-    ls = np.concatenate(([0], nl + 1)).astype(np.int64)
-    n = ls.size - 1
+    buf, ls, n = _lines(text)
     out = np.empty(buf.size + n * (AFR_MAX_FILTER_BYTES + 1) + 16, np.uint8)
     out_ls = np.empty(n + 1, np.int64)
     failed = np.empty(max(1, n), np.uint8)
@@ -894,10 +862,7 @@ def test_bsn(text: bytes, contigs: dict, params: BsnParams) -> dict:
     ugvc_test_bsn, no context): {"text", "line_start", "rescued", "hmer", "end", "n_rescued"}, or {"error": (record,
     reason)} where the reference raises."""
     lib = load_bridging_snvs()
-    buf = np.frombuffer(text, dtype=np.uint8)
-    nl = np.flatnonzero(buf == 10)  # noqa: PLR2004
-    ls = np.concatenate(([0], nl + 1)).astype(np.int64)
-    n = ls.size - 1
+    buf, ls, n = _lines(text)
     names = [k.encode() for k in contigs]
     name_buf = np.frombuffer(b"".join(names) or b"\0", dtype=np.uint8)
     name_off = np.concatenate(([0], np.cumsum([len(k) for k in names]))).astype(np.int64)
@@ -925,10 +890,7 @@ def test_hcr(text: bytes, params: HcrParams, continues_contig: bool = False, ent
     {"bed", "flags", "n_lines", "skipped", "exit_extent", "longest_segment"}, or {"error": (record, reason)} where the
     reference raises."""
     lib = load_gvcf_hcr()
-    buf = np.frombuffer(text, dtype=np.uint8)
-    nl = np.flatnonzero(buf == 10)  # noqa: PLR2004
-    ls = np.concatenate(([0], nl + 1)).astype(np.int64)
-    n = ls.size - 1
+    buf, ls, n = _lines(text)
     out = np.empty(buf.size + 48 * n + 16, np.uint8)
     flags = np.empty(max(1, n), np.uint8)
     stats = np.zeros(4, np.int64)
